@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — BASELINE.json's headline metric on B200.
+"""bench.py — BASELINE.json's headline metric on H100.
 
 Headline workload (config.workload): BASELINE config 4 — 5-term SHOULD BooleanQuery (DisjunctionSumScorer)
 BM25 top-100, batch 4096, 100M-doc synthetic Zipfian index (1M terms), evaluated by IndexSearcher::search
@@ -9,7 +9,7 @@ through the C ABI.  One "step" = one pass of the whole query batch.
   e2e    : queries/sec through rg_search_batch with HOST query arrays in and HOST TopDocs out
            (planning, H2D of the plan, kernels, D2H of results inside the timed region)
   roofline: the evaluation kernels (k_eval_or_ms + k_eval_or, or k_eval_and): algorithmic bytes per launch
-           (SURVEY 8d) / CUDA-event time, against MEASURED_PEAKS.json
+           (SURVEY 8d) / CUDA-event time, against MEASURED_PEAKS.json (else the H100 SXM data-sheet HBM3 bandwidth)
   cpu_baseline: the oracle (C++ restatement of the reference's CPU path, kind "port") timed on the box's
            usable host cores on a bounded sample of the same batch; the GPU result is checked against it
   workloads: with the default command line at N=1 also BASELINE configs 3 (2-term MUST, 10M docs) and 5
@@ -22,6 +22,10 @@ leaves per rank; every rank evaluates the whole batch on its leaves (search_para
 all-gather moves the per-leaf top-k records and every rank replays finish_parallel in leaf order.  Rank 0
 then rebuilds ALL leaves for the oracle and checks a sample, so every N carries a parity verdict.
 `--impl reference` times the oracle alone (rank 0 only).
+
+--dump-outputs DIR: after the timed steps, rank 0 writes the TopDocs of the headline workload's batch as .npy files
+(docs, scores, counts, total_hits, query_index; float64 / float32), a seeded sample of the queries when the batch's
+TopDocs exceed 64 MB.  Index and queries are generated from fixed seeds, so two builds can be compared file by file.
 """
 import argparse
 import json
@@ -56,7 +60,7 @@ WORKLOADS = {
 def parse_args():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=3)
+    ap.add_argument("--steps", type=int, default=3, help="timed steps of every leg")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="ours", choices=["ours", "reference"])
     ap.add_argument("--workload", default="c4", choices=sorted(WORKLOADS))
@@ -77,7 +81,11 @@ def parse_args():
     ap.add_argument("--stats", action="store_true", help="RG_CFG_STATS: event counters of k_eval_or_ms in the line")
     ap.add_argument("--maxscore", action="store_true",
                     help="RG_CFG_MAXSCORE: disjunctions through k_eval_or_ms (bitmaps + per-document bound) (A/B runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the TopDocs the timed path computed in its last step to DIR/<name>.npy")
     a = ap.parse_args()
+    if a.steps < 1 or a.warmup < 0:
+        ap.error("--steps must be >= 1 and --warmup >= 0")
     w = dict(WORKLOADS[a.workload])
     for key in ("docs", "terms", "batch", "k"):
         if getattr(a, key):
@@ -114,7 +122,20 @@ def measured_peaks():
             d = json.load(f)
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3), not measured"
+
+
+def device_info(index):
+    """The card's name and power limit: every absolute number of the line was measured on this."""
+    import torch
+    info = {"name": torch.cuda.get_device_name(index), "power_limit_w": None}
+    try:
+        out = subprocess.run(["nvidia-smi", "-i", str(index), "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                             stdout=subprocess.PIPE, stderr=subprocess.DEVNULL, text=True, timeout=30).stdout
+        info["power_limit_w"] = float(out.strip().splitlines()[0])
+    except Exception:
+        pass
+    return info
 
 
 class ClockSampler:
@@ -255,7 +276,7 @@ def workload_config(name, w, world):
             "name": name, "batch": w["batch"], "k": w["k"], "docs": w["docs"], "terms": w["terms"],
             "segments": n_seg, "segment_docs": seg_docs,
             "parallelism": ("%d docid-range segments, %d per GPU" % (n_seg, n_seg // world)) if n_seg > 1 else "single GPU, one segment",
-            "cache": "index image + score columns (GBs) exceed the 126 MB L2; no explicit flush"}
+            "cache": "index image + score columns (GBs) exceed the 50 MB L2 of an H100; no explicit flush"}
 
 
 # ------------------------------------------------------------------------------------------ CPU arm
@@ -318,10 +339,12 @@ def run_reference(args):
         sel = sel[np.argsort(-costs[sel], kind="stable")]
         q, c = oracle_queries(ob, [qs[i] for i in sel])
         t0 = time.perf_counter()
-        ix.search_batch(q, c, w["k"], parallel_mode=mode, n_threads=cores)
+        res = ix.search_batch(q, c, w["k"], parallel_mode=mode, n_threads=cores)
         dt = time.perf_counter() - t0
         if step >= args.warmup:
             times.append(dt)
+    if args.dump_outputs:
+        dump_outputs(args.dump_outputs, res, sel)
     ms = 1e3 * float(np.mean(times))
     value = sample / (ms / 1e3)
     line = {"impl": "reference", "metric": "queries/sec", "value": value, "unit": "queries/s",
@@ -469,7 +492,7 @@ def run_workload(ctx, name, w, args, steps, warmup, cpu_queries, cpu_seconds, fl
         b2.close()
         return res
 
-    e2e_steps = max(1, min(steps, 3))
+    e2e_steps = steps
     fresh = [build_query_arrays(gen_queries(name, w["terms"], w["batch"], w["seed_queries"] + 7919 * (i + 1)), weight_of, engine)
              for i in range(e2e_steps)]
     e2e_res = e2e_step(q, c)
@@ -559,7 +582,7 @@ def run_workload(ctx, name, w, args, steps, warmup, cpu_queries, cpu_seconds, fl
         achieved = algo_bytes / (eval_ms / 1e3) / 1e9 if eval_ms > 0 else 0.0
         out["roofline"] = {
             "bound": "hbm", "kernel": "k_eval_and" if name == "c3" else ("k_eval_or_ms (+ k_eval_or)" if flags & engine.CFG_MAXSCORE else "k_eval_or"),
-            "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": ctx.traffic.get(name),
+            "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
             "peak_source": peak_src, "algorithmic_bytes_per_launch": algo_bytes, "upper_bound_bytes_all_lists": upper_bytes,
             "kernel_ms": eval_ms,
             "replay_ms": replay_ms, "postings_per_launch": bstats["postings"], "work_items": bstats["items"],
@@ -567,7 +590,7 @@ def run_workload(ctx, name, w, args, steps, warmup, cpu_queries, cpu_seconds, fl
             "note": "algorithmic bytes = SURVEY 8d: every clause's encoded blocks + tails + 12 B/block of tables + one "
                     "norm byte per posting (conjunctions: the bytes the kernel itself counted — lead list + touched "
                     "blocks / table entries / column cells).  Dense clauses that have a score column are read from it "
-                    "(4 B per docid) instead of being decoded; traffic = DRAM bytes actually moved (ncu, profiles/)",
+                    "(4 B per docid) instead of being decoded",
             "scored_lists": dict(eng.list_stats(), note="(docid, f32 score) pairs of disjunction clauses two queries of a batch share, "
                                  "1 KB per 128-posting block; kept across batches in the engine's list arena (a ring of slabs, <= 1/6 of the free HBM)"),
             "score_columns": {"n": n_cols, "bytes": col_bytes, "built_by_first_batch": col_stats_cold["built"],
@@ -609,7 +632,7 @@ def run_workload(ctx, name, w, args, steps, warmup, cpu_queries, cpu_seconds, fl
                                     "postings_per_s": float(costs[pick].sum() / dt)}
         out["cpu_baseline"] = cpu
         del ix
-    ctx.last_engine, ctx.last_batch = eng, batch
+    ctx.last_engine, ctx.last_batch, ctx.last_result = eng, batch, result
     return out
 
 
@@ -677,12 +700,27 @@ def decode_bench(eng, stream, have_full_index):
     return res
 
 
-def load_traffic():
-    try:
-        with open(os.path.join(ROOT, "profiles", "r2_traffic.json")) as f:
-            return json.load(f)
-    except Exception:
-        return {}
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, result, query_index=None):
+    """result: (hits, counts, total) of a batch -> out_dir/{docs,scores,counts,total_hits,query_index}.npy.
+    docids and counts as float64 (exact for 32-bit integers), scores as the engine's float32.  Over
+    DUMP_LIMIT_BYTES, a fixed seeded sample of the queries (rows in batch order) is written instead."""
+    hits, counts, total = result
+    n, k = hits.shape
+    idx = np.arange(n) if query_index is None else np.asarray(query_index)
+    row_bytes = k * (8 + 4) + 3 * 8
+    budget = DUMP_LIMIT_BYTES - 4096  # room for the five .npy headers
+    if n * row_bytes > budget:
+        rows = np.sort(np.random.default_rng(0x5EED00D0).choice(n, budget // row_bytes, replace=False))
+        hits, counts, total, idx = hits[rows], counts[rows], total[rows], idx[rows]
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {"docs": hits["doc"].astype(np.float64), "scores": hits["score"].astype(np.float32),
+              "counts": counts.astype(np.float64), "total_hits": total.astype(np.float64),
+              "query_index": idx.astype(np.float64)}
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 def main():
@@ -709,8 +747,6 @@ def main():
     # exactly those launches
     ctx.stream = torch.cuda.Stream(device=ctx.dev)
     torch.cuda.set_stream(ctx.stream)
-    tr = load_traffic()
-    ctx.traffic = {} if args.scaled else {n: tr.get(n) for n in WORKLOADS}
 
     flags = ((engine.CFG_NO_COLUMNS if args.no_columns else 0) | (engine.CFG_NO_LISTS if args.no_lists else 0) |
              (engine.CFG_MAXSCORE if (args.maxscore or args.tf_planes) else 0) |
@@ -718,6 +754,8 @@ def main():
     name, w = args.workload, args.w
     main_res = run_workload(ctx, name, w, args, args.steps, args.warmup, args.cpu_sample, args.cpu_seconds, flags=flags)
     eng, batch = ctx.last_engine, ctx.last_batch
+    if ctx.rank == 0 and args.dump_outputs:
+        dump_outputs(args.dump_outputs, ctx.last_result)
     decode = None
     if ctx.rank == 0 and not args.no_decode:
         decode = decode_bench(eng, ctx.stream, have_full_index=True)
@@ -726,16 +764,16 @@ def main():
     extra = {}
     ab = {}
     if not args.no_extra and not args.scaled and name == "c4" and (flags & ~engine.CFG_STATS) == 0:
-        # A/B legs on the same workload: what the other evaluation routes deliver (2 steps each)
+        # A/B legs on the same workload: what the other evaluation routes deliver
         for label, fl in (("block_streams_only", engine.CFG_NO_COLUMNS | engine.CFG_NO_LISTS),
                           ("score_columns_no_scored_lists", engine.CFG_NO_LISTS),
                           ("bitmaps_per_document_bound", engine.CFG_MAXSCORE),
                           ("bitmaps_bound_with_tf_planes", engine.CFG_MAXSCORE | engine.CFG_TFPLANES)):
-            r = run_workload(ctx, name, w, args, 2, 1, 0, 0, flags=fl, light=True)
+            r = run_workload(ctx, name, w, args, args.steps, args.warmup, 0, 0, flags=fl, light=True)
             ab[label] = {"queries_per_s": r["value"], "ms_per_step": r["ms_per_step"]}
         if ctx.world == 1:
             for other in ("c3", "c5"):
-                r = run_workload(ctx, other, dict(WORKLOADS[other]), args, max(3, args.steps), 3, 256, 8.0)
+                r = run_workload(ctx, other, dict(WORKLOADS[other]), args, args.steps, args.warmup, 256, 8.0)
                 ctx.last_batch.close()
                 ctx.last_engine.close()
                 extra[other] = {kk: r[kk] for kk in ("value", "ms_per_step", "config", "e2e", "first_batch_ms", "roofline",
@@ -745,7 +783,7 @@ def main():
                 "steps": args.steps, "warmup": args.warmup, "ms_per_step": main_res["ms_per_step"],
                 "higher_is_better": True, "scaling": "strong", "vs_baseline": None, "dtype": "u32/f32",
                 "data": "synthetic", "config": main_res["config"], "e2e": main_res["e2e"],
-                "gpu_launches": main_res["gpu_launches"], "clocks": main_res["clocks"],
+                "gpu_launches": main_res["gpu_launches"], "device": device_info(ctx.local_rank), "clocks": main_res["clocks"],
                 "roofline": main_res.get("roofline"), "cpu_baseline": main_res.get("cpu_baseline"),
                 "first_batch_ms": main_res["first_batch_ms"], "per_rank_eval_ms": main_res["per_rank_eval_ms"],
                 "step_breakdown": {"slowest_rank_eval_kernels_ms": max(main_res["per_rank_eval_ms"]),

@@ -6,7 +6,7 @@
  * This is the "data format either side of the path": it produces real `.doc` byte streams
  * (IndexHeader + ForUtil table + per-term block/vint/skip regions + footer) that both the
  * CPU reference algorithm and the GPU engine consume.  Reference interfaces are cited per
- * function; paths are relative to /root/reference/src/core/.
+ * function; paths are relative to src/core/ of zhihu/rucene.
  */
 #ifndef RUCENE_CODEC_H
 #define RUCENE_CODEC_H

@@ -1,9 +1,9 @@
 /*
- * rucene_gpu.h — C ABI of the B200 query-evaluation engine (librucene_gpu.so).
+ * rucene_gpu.h — C ABI of the H100 query-evaluation engine (librucene_gpu.so).
  *
  * The reference (zhihu/rucene) has no FFI for this path: the hot path sits behind Rust
  * traits.  Each entry point below names the reference interface it replaces; paths are
- * relative to /root/reference/src/core/.  A Rust shim implementing `IndexSearcher<C>` binds
+ * relative to src/core/ of zhihu/rucene.  A Rust shim implementing `IndexSearcher<C>` binds
  * exactly these symbols (see INTEGRATION.md).
  *
  * Conventions: plain pointers and sizes, no exceptions across the boundary; every function
@@ -54,7 +54,7 @@ extern "C" {
 
 /* Environment variables read by the library (diagnostics / tuning sweeps; none is needed in production):
  * RG_PLAN_TIMING=1 prints where rg_batch_prepare's host time goes; RG_OR_COL_DEN=n reads a disjunction clause from its
- * score column when df >= max_doc/n (default 16); RG_MAX_RANGES=n caps the docid ranges per (query, leaf) (default 128);
+ * score column when df >= max_doc/n (default 8); RG_MAX_RANGES=n caps the docid ranges per (query, leaf) (default 256);
  * RG_LIST_ARENA_KB=n sizes the scored-list arena (default: a sixth of the free HBM, at most 24 GiB). */
 
 typedef struct rg_engine rg_engine;

@@ -2,7 +2,7 @@
  * oracle.cpp — CPU restatement of zhihu/rucene's IndexSearcher hot path.
  *
  * TEST INFRASTRUCTURE ONLY (see oracle.h).  Every function cites the reference
- * file:line it follows; paths are relative to /root/reference/src/core/.
+ * file:line it follows; paths are relative to src/core/ of zhihu/rucene.
  * Compile with -ffp-contract=off: the reference (rustc) never contracts a*b+c
  * into an FMA and BM25 bit-exactness depends on that.
  *

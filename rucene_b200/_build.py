@@ -1,6 +1,6 @@
 """In-tree builds of the native libraries (no JIT cache: the .so files travel with the repo).
 
-librucene_gpu.so   : CUDA kernels + the C ABI of include/rucene_gpu.h   (nvcc, sm_100a)
+librucene_gpu.so   : CUDA kernels + the C ABI of include/rucene_gpu.h   (nvcc, sm_90a)
 librucene_codec.so : host write side / BM25 host math / synthetic index (g++)
 
 (The CPU checker under oracle/ is test infrastructure with its own Makefile; nothing in this
@@ -17,7 +17,7 @@ INC = os.path.join(ROOT, "include")
 
 HOST_FLAGS = ["-O3", "-march=x86-64-v3", "-std=c++17", "-fPIC", "-ffp-contract=off", "-Wall",
               "-Wextra", "-pthread"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC,-ffp-contract=off,-pthread", "--fmad=false", "-prec-div=true",
               "-prec-sqrt=true", "-Xptxas", "-v"]
 

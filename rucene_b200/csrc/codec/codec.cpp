@@ -1,7 +1,7 @@
 // codec.cpp — host-side write path of the Lucene50 postings format (DocsAndFreqs field),
 // BM25 weight helpers and the synthetic Zipfian index generator (librucene_codec.so).
 //
-// Format references (paths relative to /root/reference/src/core/):
+// Format references (paths relative to src/core/ of zhihu/rucene):
 //   codec/postings/posting_writer.rs:289-361,457-474,477-589   term/doc/block emission
 //   codec/postings/skip_writer.rs:187-290                       multi-level skip data
 //   codec/postings/for_util.rs:150-185,374-478                  ForUtil table + write_block

@@ -1,4 +1,4 @@
-// common.cuh — shared device/host definitions of the B200 query-evaluation engine.
+// common.cuh — shared device/host definitions of the H100 query-evaluation engine.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

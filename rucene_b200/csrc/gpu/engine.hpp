@@ -287,8 +287,9 @@ struct rg_engine {
     std::deque<ListSlab> list_slabs;
     bool list_arena_tried = false;
     // the exhaustive disjunction kernel scans a score column docid by docid: that beats streaming the clause's postings
-    // (scored list) for df >= max_doc / or_col_den; measured on C4: 1/8 342 ms, 1/16 331, 1/32 336, 1/64 351
-    uint64_t or_col_den = 16;
+    // (scored list) for df >= max_doc / or_col_den; measured on C4 (one H100 at 400 W, 256 ranges per leaf):
+    // 1/4 641 ms, 1/8 627, 1/16 669 per step
+    uint64_t or_col_den = 8;
     bool range_postings_set = false;  // rg_config.range_postings was given (else the planner chooses per batch)
     uint64_t generation = 1;            // bumped by rg_segment_upload / rg_norm_cache_set (stale-batch check)
     std::vector<uint8_t> cache_nonneg;  // per norm cache: every entry >= 0 (MaxScore bound needs it)

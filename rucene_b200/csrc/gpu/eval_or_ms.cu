@@ -1,5 +1,5 @@
 // eval_or_ms.cu — k_eval_or_ms: pure-SHOULD sum disjunctions (DisjunctionSumScorer, TermScorer) over
-// presence bitmaps, score columns and a bit-sliced per-document score bound.  sm_100a, integer/HBM work.
+// presence bitmaps, score columns and a bit-sliced per-document score bound.  sm_90a, integer/HBM work.
 //
 // What the reference computes (search/scorer/disjunction_scorer.rs:187-244, bulk_scorer.rs:89-122,
 // collector/top_docs.rs:67-95) is, per (query, leaf): total_hits = |union of the clauses' live docs| and the

@@ -1,4 +1,4 @@
-// query_kernels.cu — the fused query-evaluation kernels (sm_100a, integer/HBM-bound work).
+// query_kernels.cu — the fused query-evaluation kernels (sm_90a, integer/HBM-bound work).
 //
 //   k_build_columns: batch-level common subexpression — the BM25 contributions of a dense clause that
 //                 several disjunctions of the batch share, computed once into a docid-indexed f32 column.

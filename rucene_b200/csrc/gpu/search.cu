@@ -699,13 +699,13 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
     }
     // Docid ranges (= work items) per (query, leaf).  A caller's rg_config.range_postings is taken as is: ~that many
     // postings per range.  By default conjunction items (one CTA each) get 32 K postings; disjunctions (one warp each)
-    // are cut on a GRID THE WHOLE BATCH SHARES: per leaf a power of two R_leaf <= 128 of equal docid ranges, sized so that
+    // are cut on a GRID THE WHOLE BATCH SHARES: per leaf a power of two R_leaf <= 256 of equal docid ranges, sized so that
     // an average query's range holds ~128 K postings (longer ranges cost less setup and keep theta chains short) but the
     // batch still has ~32 K items; an inexpensive query takes R_leaf / 2^j of them (>= 8 K postings each).  Items are
     // launched in order of their range's start on that grid, so the warps in flight read the same region of the
-    // columns, lists and norms through L2 — measured on C4 (one 100 M-doc leaf): 128 equal ranges 318 ms, 256 324,
-    // 512 334, and 343 with range counts that differ from query to query.
-    static const uint64_t max_ranges = getenv("RG_MAX_RANGES") ? std::max(1, atoi(getenv("RG_MAX_RANGES"))) : 128;  // tuning knob
+    // columns, lists and norms through L2 — measured on C4 (one 100 M-doc leaf, one H100 at 400 W, columns for
+    // df >= max_doc/8): 128 equal ranges 670 ms, 256 627, 512 627.
+    static const uint64_t max_ranges = getenv("RG_MAX_RANGES") ? std::max(1, atoi(getenv("RG_MAX_RANGES"))) : 256;  // tuning knob
     uint64_t and_rp = e->cfg.range_postings, or_rp = e->cfg.range_postings;
     std::vector<uint32_t> or_grid(n_segs, 0);  // R_leaf; 0 = per-query ranges of or_rp postings (explicit range_postings)
     if (!e->range_postings_set) {

@@ -5,7 +5,7 @@
 // query kernels).  Payload parts are 16-byte aligned in the HBM image (common.cuh), which makes
 // every load a 128-bit (SIMD128 layout) or aligned 32-bit (big-endian layouts) access.
 //
-// Reference semantics (paths relative to /root/reference/src/core/):
+// Reference semantics (paths relative to src/core/ of zhihu/rucene):
 //   SIMD128 (".doc" version 1): util/packed/packed_simd.rs:126-163 unpack_bits!
 //       value n -> lane l = n%4, lane-stream slot q = n/4; v = (W[j][l] >> s | W[j+1][l] << (32-s))
 //       & mask with j = q*b/32, s = q*b%32 over little-endian words.

@@ -2,7 +2,7 @@
 // (query term) before any posting is touched.  Product code (used by librucene_codec.so and
 // by the C++ searcher mirror); independent of oracle/.
 //
-// Reference (paths relative to /root/reference/src/core/):
+// Reference (paths relative to src/core/ of zhihu/rucene):
 //   util/small_float.rs:16-36                         byte315 <-> f32
 //   search/similarity/bm25_similarity.rs:33-43        NORM_TABLE
 //   search/similarity/bm25_similarity.rs:72-83        avg_field_length

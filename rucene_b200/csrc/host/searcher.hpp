@@ -8,7 +8,7 @@
 //   search/collector/top_docs.rs:107-124 TopDocsCollector::new(k) / top_docs()
 //   search/sort_field/collapse_top_docs.rs:22-68,288-326 ScoreDoc / TopDocs
 //   search/similarity/bm25_similarity.rs:45-46,151-177 BM25Similarity, compute_weight
-// (paths relative to /root/reference/src/core/).  Header-only; link librucene_gpu.so.
+// (paths relative to src/core/ of zhihu/rucene).  Header-only; link librucene_gpu.so.
 #pragma once
 #include <cstdint>
 #include <memory>

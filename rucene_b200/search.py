@@ -1,7 +1,7 @@
 """Python mirror of the reference's search surface for the accelerated path.
 
 Same names and argument meaning as the Rust reference (paths relative to
-/root/reference/src/core/):
+src/core/ of zhihu/rucene):
 
     Term                 index/mod.rs Term::new(field, bytes)
     TermQuery            search/query/term_query.rs:46-49    TermQuery::new(term, boost, ctx)
@@ -187,7 +187,7 @@ class IndexReader:
 
 
 class GpuIndexSearcher:
-    """IndexSearcher<C> whose search() runs on the B200 (DefaultIndexSearcher::new(reader, None))."""
+    """IndexSearcher<C> whose search() runs on the H100 (DefaultIndexSearcher::new(reader, None))."""
 
     def __init__(self, reader: IndexReader, similarity: Optional[BM25Similarity] = None,
                  device=-1, eng: Optional[engine.Engine] = None, range_postings=0,

@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Summarise one kernel of an .ncu-rep into the JSON kept under profiles/.
+"""Summarise one kernel of an .ncu-rep into JSON.
 
-usage: ncu_summary.py <report.ncu-rep> <kernel-name-substring> <note> > profiles/<name>_summary.json
-Reads `ncu -i … --page raw --csv`; keeps the metrics the DESIGN / profiles README quote.
+usage: ncu_summary.py <report.ncu-rep> <kernel-name-substring> <note> > <name>_summary.json
+Reads `ncu -i … --page raw --csv`; keeps the time, DRAM, instruction and pipe metrics of the kernel.
 """
 import csv, io, json, subprocess, sys
 

@@ -43,9 +43,9 @@ def test_engine_fails_loudly_without_a_device():
     assert "no CPU fallback" in str(ei.value)
 
 
-def test_gpu_library_targets_sm_100a():
+def test_gpu_library_targets_sm_90a():
     import shutil
     import subprocess
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
     out = subprocess.run([cuobjdump, "-lelf", _build.build_gpu()], stdout=subprocess.PIPE, text=True).stdout
-    assert "sm_100a" in out
+    assert "sm_90a" in out

@@ -1,6 +1,6 @@
 """The oracle pinned against every known-answer vector the reference's own tests hold for the
 hot path (SURVEY.md §4 / §8c).  Each test names the reference test it transcribes
-(paths relative to /root/reference/src/core/).  CPU only."""
+(paths relative to src/core/ of zhihu/rucene).  CPU only."""
 import math
 
 import numpy as np
