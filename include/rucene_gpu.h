@@ -213,7 +213,8 @@ int rg_batch_stats(rg_engine* e, rg_batch* b, uint64_t out[8]);
  * the bit-sliced bound, [3]=windows before any theta, [4]=docids only counted (between windows), [5]=stream postings
  * visited, [6]=column gathers, [7]=block refills, [8]=candidates, [9]=32-doc steps scanned for candidates,
  * [10]=windows cut by a sparse stream's cache end, [11]=windows with a non-empty scoring set, [12]=docs scored.
- * Always counted (no flag needed): [15]=bytes the conjunction kernel (k_eval_and) asked for in the last run —
+ * Always counted (no flag needed): [14]=work items the planner sent to the decode-free k_eval_or (every clause a
+ * score column or a scored list; known from rg_batch_prepare on), [15]=bytes the conjunction kernel (k_eval_and) asked for in the last run —
  * decoded block parts + 12 B of tables per block, 4 B per skip probe and column gather, 1 norm byte per scored
  * posting: the "touched blocks" figure of its roofline. */
 int rg_batch_debug(rg_engine* e, rg_batch* b, uint64_t out[16]);

@@ -600,6 +600,7 @@ void build_segment(rg_engine* e, Segment& seg, int32_t doc_base, int32_t max_doc
         }
     seg.n_blocks_total = n_blocks;
     e->col_budget_floats = 0;
+    e->local_budget_floats = 0;
     seg.doc_base = doc_base;
     seg.max_doc = max_doc;
     seg.dev.arena = seg.arena.p;

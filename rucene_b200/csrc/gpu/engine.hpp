@@ -212,6 +212,8 @@ void launch_build_tf_planes(cudaStream_t st, const SegDev* segs, const ColumnJob
 void refresh_cache_small(rg_engine* e);
 void launch_eval_or(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n,
                     uint32_t max_terms, bool has_live, bool has_not, bool has_msm, bool has_dmax, bool all_pos);
+// the decode-free k_eval_or: plain-sum items whose every clause is a score column or a scored list
+void launch_eval_or_lean(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n, bool has_live);
 // eval_dpq.cu: disjunctions with >= 10 clauses in a leaf (DisiPriorityQueue order), one warp per (query, leaf)
 void launch_eval_dpq(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n, uint32_t max_terms,
                      bool has_live);
@@ -268,6 +270,7 @@ struct rg_engine {
     std::map<rg::ColKey, std::shared_ptr<rg::ColEntry>> col_cache;
     uint64_t col_floats = 0;            // floats held by map-resident entries
     uint64_t col_budget_floats = 0;     // 0 = not computed yet (reset by rg_segment_upload)
+    uint64_t local_budget_floats = 0;   // batch-local scored lists per batch (search.cu), likewise
     uint64_t col_tick = 0, col_builds = 0, col_hits = 0;
     // persistent scored posting lists (same key, same budget and LRU clock as the columns)
     std::map<rg::ColKey, std::shared_ptr<rg::ColEntry>> list_cache;

@@ -283,7 +283,7 @@ k_eval_dpq(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, 
                 }
             }
             __syncwarp();
-            wtheta_update(em, p.k, kcap, lane, sh.newc, newc_n, p.item_theta + item_idx);
+            wtheta_update(em, p, item_idx, kcap, lane, sh.newc, newc_n);
             __syncwarp();
             if (lane == 0) st.nout = 0;
         }

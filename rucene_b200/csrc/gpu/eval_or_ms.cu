@@ -551,7 +551,7 @@ k_eval_or_ms(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids
             // re-arm the accumulator words that were touched (E bits live in the owning lane's word)
             if ((uint32_t)lane < n_e) sh.acc[lane] = 0.0f;
             if ((uint32_t)lane + 32u < n_e) sh.acc[lane + 32] = 0.0f;
-            wtheta_update(em, p.k, kcap, lane, sh.newc, newc_n, p.item_theta + item_idx);
+            wtheta_update(em, p, item_idx, kcap, lane, sh.newc, newc_n);
             __syncwarp();
         }
         pos = win1;

@@ -268,10 +268,10 @@ struct WTerm {
     const int32_t* blk_last;
     const BlockDesc* blk_desc;
     const float* cache;
-    uint32_t nb;        // full blocks
-    uint32_t cur;       // next block to decode (nb = vint tail, nb+1 = exhausted)
+    uint32_t nb;        // full blocks; decode-free variant (LEAN): units of the scored list, full blocks + the tail if any
+    uint32_t cur;       // next block to decode (nb = vint tail, nb+1 = exhausted); LEAN: the cursor's unit, nb = exhausted
     uint32_t n;         // valid entries in the stream cache
-    uint32_t pos;       // next unconsumed entry
+    uint32_t pos;       // next unconsumed entry (LEAN: within unit cur of the scored list)
     uint32_t term_id;
     float w1;           // weight * (k1 + 1)
     uint32_t is_not;    // MUST_NOT clause: its postings exclude docs (search/scorer/req_not_scorer.rs)
@@ -331,8 +331,8 @@ struct alignas(16) WarpShared {  // followed by topk[kcap] floats, then cdocs[T]
 // warp-level candidate emitter state (registers, uniform across lanes)
 struct WEmit {
     float* topk;       // shared memory, kcap floats
-    float* gtopk;      // global mirror of topk (EvalParams::item_topk row of this item), null = not kept
-    uint32_t* gcount;  // its published entry count
+    bool mirror;       // topk is mirrored into EvalParams::item_topk[item] and its count into item_topk_n[item]
+                       // (formed from the params at each use: a pointer pair held across the window loop costs registers)
     uint32_t topk_n;
     float theta_local;
     uint32_t theta_in;
@@ -364,10 +364,12 @@ __device__ __forceinline__ void wtheta_recompute(const WEmit& em, uint32_t k, in
     argmin = mi;
 }
 
-__device__ __forceinline__ void wtheta_update(WEmit& em, uint32_t k, uint32_t kcap, int lane,
-                                              const float* newc, uint32_t newc_n, uint32_t* theta_out) {
+__device__ __forceinline__ void wtheta_update(WEmit& em, const EvalParams& p, uint32_t item_idx, uint32_t kcap, int lane,
+                                              const float* newc, uint32_t newc_n) {
+    const uint32_t k = p.k;
     const uint32_t n_new = min(newc_n, (uint32_t)kNewcW);
     if (n_new == 0 || k > kcap) return;
+    float* gtopk = em.mirror ? p.item_topk + (size_t)item_idx * kcap : nullptr;
     __syncwarp();
     float theta = em.theta_local;
     int argmin = 0;
@@ -378,7 +380,7 @@ __device__ __forceinline__ void wtheta_update(WEmit& em, uint32_t k, uint32_t kc
         if (n < k) {
             if (lane == 0) {
                 em.topk[n] = x;
-                if (em.gtopk) em.gtopk[n] = x;
+                if (gtopk) gtopk[n] = x;
             }
             n++;
             __syncwarp();
@@ -386,7 +388,7 @@ __device__ __forceinline__ void wtheta_update(WEmit& em, uint32_t k, uint32_t kc
         } else if (x > theta) {
             if (lane == 0) {
                 em.topk[argmin] = x;
-                if (em.gtopk) em.gtopk[argmin] = x;
+                if (gtopk) gtopk[argmin] = x;
             }
             __syncwarp();
             wtheta_recompute(em, k, lane, theta, argmin);
@@ -396,13 +398,13 @@ __device__ __forceinline__ void wtheta_update(WEmit& em, uint32_t k, uint32_t kc
     em.topk_n = n;
     em.theta_local = n == k ? theta : -INFINITY;
     if (lane == 0) {
-        if (em.gcount && grew) {  // entries first, then the count a successor reads
+        if (em.mirror && grew) {  // entries first, then the count a successor reads
             __threadfence();
-            *reinterpret_cast<volatile uint32_t*>(em.gcount) = n;
+            *reinterpret_cast<volatile uint32_t*>(p.item_topk_n + item_idx) = n;
         }
         uint32_t ord = em.theta_in;
         if (em.theta_local != -INFINITY) ord = max(ord, float_to_ordered(em.theta_local));
-        if (ord > kOrderedNegInf) atomicMax(theta_out, ord);
+        if (ord > kOrderedNegInf) atomicMax(p.item_theta + item_idx, ord);
     }
 }
 
@@ -414,12 +416,9 @@ __device__ __forceinline__ void wtheta_update(WEmit& em, uint32_t k, uint32_t kc
 // score, far below the root of a heap that has seen hundreds of ranges.
 __device__ __forceinline__ void wtheta_inherit(WEmit& em, const EvalParams& p, uint32_t item_idx, uint32_t chain_pos,
                                                uint32_t kcap, int lane) {
-    em.gtopk = nullptr;
-    em.gcount = nullptr;
-    if (!p.item_topk || p.k > kcap) return;
-    em.gtopk = p.item_topk + (size_t)item_idx * kcap;
-    em.gcount = p.item_topk_n + item_idx;
-    if (chain_pos == 0) return;
+    em.mirror = p.item_topk && p.k <= kcap;
+    if (!em.mirror || chain_pos == 0) return;
+    float* gtopk = p.item_topk + (size_t)item_idx * kcap;
     uint32_t cnt = 0;
     if ((uint32_t)lane < chain_pos) cnt = ld_volatile_u32(p.item_topk_n + item_idx - 1 - lane);
     const uint32_t have = __ballot_sync(0xffffffffu, cnt > 0u);
@@ -431,7 +430,7 @@ __device__ __forceinline__ void wtheta_inherit(WEmit& em, const EvalParams& p, u
     for (uint32_t j = lane; j < n; j += 32) {
         const float v = __uint_as_float(ld_volatile_u32(reinterpret_cast<const uint32_t*>(src + j)));
         em.topk[j] = v;
-        em.gtopk[j] = v;
+        gtopk[j] = v;
     }
     __syncwarp();
     em.topk_n = n;
@@ -443,7 +442,7 @@ __device__ __forceinline__ void wtheta_inherit(WEmit& em, const EvalParams& p, u
     }
     if (lane == 0) {
         __threadfence();
-        *reinterpret_cast<volatile uint32_t*>(em.gcount) = n;
+        *reinterpret_cast<volatile uint32_t*>(p.item_topk_n + item_idx) = n;
         if (em.theta_local != -INFINITY) atomicMax(p.item_theta + item_idx, float_to_ordered(em.theta_local));
     }
 }

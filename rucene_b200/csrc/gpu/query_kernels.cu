@@ -162,10 +162,60 @@ __device__ __noinline__ uint32_t columns_only_window(const WTerm* term, uint32_t
     return __any_sync(0xffffffffu, mx > te) ? 0xffffffffu : c;
 }
 
-template <bool LIVE, bool NOT, bool MSM, bool DMAX, bool POS>
-__global__ void __launch_bounds__(kOrThreads, 24)
+// One scored-list clause over the window [win0, win1) of the decode-free variant: the list is read straight from global
+// memory at the clause's (block, position) cursor.  A block that lies inside the window is two 16-byte loads per lane;
+// one that straddles windows is consumed 32 entries per step (re-read from L1 in the next window).  Every entry at or
+// after the cursor is >= lo, and the tail unit's entries past the end hold kNoMoreDocs.  Returns the clause's next
+// docid (kNoMoreDocs when nothing is left below hi).
+__device__ __forceinline__ int list_window(uint32_t* acc, WTerm& tc, int win0, int win1, int hi, int lane) {
+    const uint32_t* list = reinterpret_cast<const uint32_t*>(tc.pre);
+    const uint32_t nb = tc.nb;  // units holding postings: full blocks + the tail, if any
+    uint32_t b = tc.cur, pos = tc.pos;
+    int nx = kNoMoreDocs;
+    while (b < nb) {
+        const uint32_t* blk = list + (size_t)b * (2 * kBlock);
+        if (pos == 0 && (int)__ldg(blk + kBlock - 1) < win1) {
+            const uint4 dv = __ldg(reinterpret_cast<const uint4*>(blk) + lane);
+            const uint4 sv = __ldg(reinterpret_cast<const uint4*>(blk) + 32 + lane);
+            if (b + 1 < nb && lane < 8) asm volatile("prefetch.global.L2 [%0];" ::"l"(blk + 2 * kBlock + lane * 32));
+            const uint32_t d[4] = {dv.x, dv.y, dv.z, dv.w}, s[4] = {sv.x, sv.y, sv.z, sv.w};
+#pragma unroll
+            for (int q = 0; q < 4; q++) {
+                uint32_t* a = acc + ((int)d[q] - win0);
+                *a = __float_as_uint(__fadd_rn(__uint_as_float(*a), __uint_as_float(s[q])));
+            }
+            b++;
+            continue;
+        }
+        const uint32_t i = pos + lane;
+        const int d = i < (uint32_t)kBlock ? (int)__ldg(blk + i) : kNoMoreDocs;
+        const float s = i < (uint32_t)kBlock ? __uint_as_float(__ldg(blk + kBlock + i)) : 0.0f;
+        const bool in_win = d < win1;
+        const uint32_t c = __popc(__ballot_sync(0xffffffffu, in_win));  // sorted: a prefix
+        if (in_win) acc[d - win0] = __float_as_uint(__fadd_rn(__uint_as_float(acc[d - win0]), s));
+        pos += c;
+        if (pos == (uint32_t)kBlock) {
+            b++;
+            pos = 0;
+        } else if (c < 32) {
+            nx = __shfl_sync(0xffffffffu, d, c);  // the entry at the new cursor
+            break;
+        }
+    }
+    if (nx >= hi) b = nb;
+    // every lane stores the same cursor and later reads back its own store
+    tc.cur = b;
+    tc.pos = pos;
+    return b < nb ? nx : kNoMoreDocs;
+}
+
+// LEAN: the decode-free variant for plain-sum items (POS) whose every clause is a score column or a scored list —
+// no block decode, no stream cache in shared memory, so fewer registers and more resident warps.
+template <bool LIVE, bool NOT, bool MSM, bool DMAX, bool POS, bool LEAN = false>
+__global__ void __launch_bounds__(kOrThreads, LEAN ? 32 : 24)
 k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, uint32_t warp_bytes,
           uint32_t kcap) {
+    static_assert(!LEAN || (POS && !NOT && !MSM && !DMAX), "the decode-free variant is plain-sum only");
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int lane = lane_id(), warp = threadIdx.x >> 5;
     const uint32_t wid = blockIdx.x * kOrWarps + warp;
@@ -218,7 +268,7 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
         tc.blk_last = seg.blk_last + td.blk_begin;
         tc.blk_desc = seg.blk_desc + td.blk_begin;
         tc.cache = p.caches + (size_t)c.cache_id * 256;
-        tc.nb = td.n_blocks;
+        tc.nb = LEAN ? td.n_blocks + (td.tail_n ? 1u : 0u) : td.n_blocks;
         tc.cur = lower_bound_i32(tc.blk_last, 0, td.n_blocks, lo);
         tc.n = 0;
         tc.pos = 0;
@@ -227,10 +277,23 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
         tc.is_not = c.flags & 1u;
     }
     __syncwarp();
-    const uint32_t col_mask = __ballot_sync(0xffffffffu, lane < T && sh.term[lane < T ? lane : 0].is_col != 0);
+    const bool my_stream = lane < T && sh.term[lane < T ? lane : 0].is_col == 0;  // lane t: clause t is not a column
     uint32_t hot = 0, my_matches = 0;
     int nd = kNoMoreDocs;  // lane t: next cached docid of clause t (kNoMoreDocs = exhausted)
-    for (int t = 0; t < T; t++) {
+    for (int t = 0; t < T && LEAN; t++) {
+        // scored list: put the cursor on the first posting >= lo of the block the skip table found
+        WTerm& tc = sh.term[t];
+        if (tc.is_col || tc.cur >= tc.nb) continue;
+        const uint32_t* blk = reinterpret_cast<const uint32_t*>(tc.pre) + (size_t)tc.cur * (2 * kBlock);
+        const uint4 dv = __ldg(reinterpret_cast<const uint4*>(blk) + lane);
+        const uint32_t pos = __reduce_add_sync(0xffffffffu, ((int)dv.x < lo) + ((int)dv.y < lo) + ((int)dv.z < lo) +
+                                                                ((int)dv.w < lo));
+        const int first = (int)__ldg(blk + pos);  // pos < kBlock: the block's last docid (or a tail pad) is >= lo
+        __syncwarp();
+        tc.pos = pos;
+        if (lane == t) nd = first < hi ? first : kNoMoreDocs;
+    }
+    for (int t = 0; t < T && !LEAN; t++) {
         if (stream_refill<LIVE, NOT, MSM, DMAX, POS>(seg, p, sh.term[t], cdocs + t * kBlock, cscores + t * kBlock, lo, hi,
                                                 lane, 0, -2147483647 - 1, sh.acc, hot, my_matches, INFINITY, mc)) {
             const int first = cdocs[t * kBlock + sh.term[t].pos];
@@ -240,7 +303,7 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
     // a column clause has a (potential) posting at every docid: windows become contiguous and
     // 4-aligned (16-byte column loads) from the start of the range
     if (lane < T && sh.term[lane].is_col && lo < hi) nd = lo & ~3;
-    long long w0 = __reduce_min_sync(0xffffffffu, nd);
+    int w0 = __reduce_min_sync(0xffffffffu, nd);
 
     WEmit em;
     em.topk = topk;
@@ -256,15 +319,14 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
     // theta look-back: the up-to-32 preceding items of this heap chain (each publishes
     // max(own, inherited)), re-read every 8 windows
     const bool lb_ok = (uint32_t)lane < it.chain_pos;
-    const uint32_t* theta_lb = p.item_theta + item_idx - 1 - (lb_ok ? lane : 0);
     uint32_t win_no = 0;
 
     while (w0 < hi) {
-        const int win0 = (int)w0;
-        const int win1 = (int)min((long long)hi, w0 + kWw);
+        const int win0 = w0;
+        const int win1 = hi - win0 > kWw ? win0 + kWw : hi;
         uint32_t inherited = 0;
         if ((win_no++ & 7u) == 0 && it.chain_pos) {
-            inherited = lb_ok ? ld_volatile_u32(theta_lb) : 0u;
+            inherited = lb_ok ? ld_volatile_u32(p.item_theta + item_idx - 1 - lane) : 0u;
             inherited = __reduce_max_sync(0xffffffffu, inherited);
         }
         hot = 0;
@@ -281,7 +343,7 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
         // ---- clauses with a posting in this window, in clause order: drain each stream up to the
         // window end (a sparse clause sits out most windows)
         uint32_t active = __ballot_sync(0xffffffffu, nd < win1);
-        if (POS && active && (active & ~col_mask) == 0u && win1 - win0 == kWw && win0 >= lo) {
+        if (POS && active && !__any_sync(0xffffffffu, my_stream && nd < win1) && win1 - win0 == kWw && win0 >= lo) {
             // Only score columns have postings in this (whole) window: see columns_only_window.  Only if a doc beats
             // theta (rare) the general path below redoes the window to scan it.
             const uint32_t cnt = columns_only_window<LIVE>(sh.term, active, seg.live, win0, hi, te, lane);
@@ -327,6 +389,12 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
                 }
                 if (lane == t) nd = win1 < hi ? win1 : kNoMoreDocs;
                 __syncwarp();
+                continue;
+            }
+            if (LEAN) {
+                const int nx = list_window(sh.acc, tc, win0, win1, hi, lane);
+                if (lane == t) nd = nx;
+                __syncwarp();  // the next clause's lanes read window slots other lanes have just written
                 continue;
             }
             const int32_t* cd = cdocs + t * kBlock;
@@ -437,7 +505,7 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
             if (MSM) {
                 for (int i = lane; i < kWw / 16; i += 32) reinterpret_cast<uint4*>(mc.cnt)[i] = make_uint4(0, 0, 0, 0);
             }
-            wtheta_update(em, p.k, kcap, lane, sh.newc, newc_n, p.item_theta + item_idx);
+            wtheta_update(em, p, item_idx, kcap, lane, sh.newc, newc_n);
             __syncwarp();
         }
         if (next_doc == kNoMoreDocs) break;
@@ -1081,14 +1149,22 @@ void launch_build_tf_planes(cudaStream_t st, const SegDev* segs, const ColumnJob
     if (hist) k_build_columns<3><<<ctas, kColWarps * 32, 0, st>>>(segs, jobs, n_jobs, n_units, caches, k1, hist, 0);
     else k_build_columns<2><<<ctas, kColWarps * 32, 0, st>>>(segs, jobs, n_jobs, n_units, caches, k1, nullptr, plane_stride);
 }
-template <bool LIVE, bool NOT, bool MSM, bool DMAX, bool POS = false>
+template <bool LIVE, bool NOT, bool MSM, bool DMAX, bool POS = false, bool LEAN = false>
 static void launch_eval_or_t(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n, size_t wb,
                              uint32_t kcap) {
     const size_t smem = wb * kOrWarps;
     // per launch, not cached: the attribute is per device and engines may live on several
-    cudaFuncSetAttribute(k_eval_or<LIVE, NOT, MSM, DMAX, POS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(k_eval_or<LIVE, NOT, MSM, DMAX, POS, LEAN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     const uint32_t ctas = (n + kOrWarps - 1) / kOrWarps;
-    k_eval_or<LIVE, NOT, MSM, DMAX, POS><<<ctas, kOrThreads, smem, st>>>(p, item_ids, n, (uint32_t)wb, kcap);
+    k_eval_or<LIVE, NOT, MSM, DMAX, POS, LEAN><<<ctas, kOrThreads, smem, st>>>(p, item_ids, n, (uint32_t)wb, kcap);
+}
+// plain-sum items whose every clause is a score column or a scored list (no stream cache in shared memory)
+void launch_eval_or_lean(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n, bool has_live) {
+    if (!n) return;
+    const uint32_t kcap = (std::min<uint32_t>(p.k, kMaxK) + 31u) & ~31u;
+    const size_t wb = (sizeof(WarpShared) + (size_t)kcap * sizeof(float) + 15) & ~size_t(15);
+    if (has_live) launch_eval_or_t<true, false, false, false, true, true>(st, p, item_ids, n, wb, kcap);
+    else launch_eval_or_t<false, false, false, false, true, true>(st, p, item_ids, n, wb, kcap);
 }
 // has_live: some leaf has deleted docs; has_not: some item of the launch carries a MUST_NOT clause;
 // all_pos: every clause score of every item of the launch is > 0 (the planner checked weights and norm caches)

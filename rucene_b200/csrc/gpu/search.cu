@@ -47,6 +47,9 @@ struct rg_batch {
     Span<ItemClause> clauses;
     Span<uint32_t> or_ids, and_ids;  // launch order (range-major) of the OR / AND work items
     Span<uint32_t> ms_ids;           // OR work items evaluated by k_eval_or_ms (bitmaps + non-essential clauses)
+    Span<uint32_t> lean_ids;         // OR work items of the decode-free k_eval_or (every clause a column / scored list)
+    uint32_t n_lean = 0;
+    Span<uint4> local_lists;         // batch-local scored lists (choose_local_lists), built by rg_batch_prepare
     Span<uint32_t> dpq_ids;          // disjunctions with >= 10 clauses in the leaf (k_eval_dpq), one per (query, leaf)
     uint32_t n_dpq = 0, max_dpq_terms = 0;
     bool uses_planes = false;        // some column / bitmap reference of this batch carries tf-norm planes
@@ -73,6 +76,7 @@ struct rg_batch {
     uint32_t kernels_per_run = 0;
     bool or_has_not = false, or_has_msm = false, or_has_dmax = false, or_nonpos = false;
     bool ran = false;
+    bool local_built = false;  // batch-local scored lists were launched into the slab
     // two batches may be in flight (prepare the next while one runs): the plan goes up on the engine's copy stream,
     // the run waits for `uploaded`, the fetch waits for `done` on the copy stream; timing events are the batch's own
     cudaEvent_t uploaded = nullptr, done = nullptr, ev[4] = {nullptr, nullptr, nullptr, nullptr};
@@ -106,14 +110,20 @@ struct PlanTimer {
 struct HostPlan {
     std::vector<WorkItem> items;
     std::vector<ItemClause> clauses;
-    std::vector<uint32_t> or_ids, ms_ids, and_ids, ro_ids, dpq_ids;
+    std::vector<uint32_t> or_ids, ms_ids, and_ids, ro_ids, dpq_ids, lean_ids;
     uint32_t max_dpq_terms = 0;
+    // batch-local scored lists: build jobs whose dst is an offset (in floats) into the batch's list region, and the
+    // col_refs entries to point there once the slab exists
+    std::vector<ColumnJob> local_jobs;
+    std::vector<std::pair<uint32_t, uint64_t>> local_refs;  // (col_refs index, offset in floats)
+    uint64_t local_floats = 0;
+    uint32_t local_units = 0;
     std::vector<ColRef> col_refs;
     std::map<std::tuple<uint32_t, uint32_t, uint32_t>, uint32_t> bitmap_refs;  // (leaf, term, cache) -> col_refs entry {null, bits, hi}
     std::vector<std::shared_ptr<ColEntry>> cols, lists;
     uint32_t n_cols_built = 0, n_lists_built = 0, max_ms_streams = 0;
     uint64_t col_floats = 0, list_floats = 0;
-    std::vector<uint32_t> or_rank, ms_rank, and_rank;  // range index of each id (launch-order key)
+    std::vector<uint32_t> or_rank, ms_rank, and_rank, lean_rank;  // range index of each id (launch-order key)
     std::vector<uint32_t> group_item_begin, group_out;
     uint64_t postings = 0, algo_bytes = 0;
     uint32_t max_or_terms = 1;
@@ -122,6 +132,9 @@ struct HostPlan {
     // in by every rg_batch_prepare)
     void reset() {
         items.clear(); clauses.clear(); or_ids.clear(); ms_ids.clear(); and_ids.clear(); ro_ids.clear(); dpq_ids.clear();
+        lean_ids.clear(); lean_rank.clear(); local_jobs.clear(); local_refs.clear();
+        local_floats = 0;
+        local_units = 0;
         col_refs.clear(); bitmap_refs.clear(); cols.clear(); lists.clear(); or_rank.clear(); ms_rank.clear(); and_rank.clear();
         group_item_begin.clear(); group_out.clear();
         max_dpq_terms = n_cols_built = n_lists_built = max_ms_streams = 0;
@@ -682,6 +695,98 @@ std::map<ColKey, uint32_t> choose_lists(rg_engine* e, const std::vector<QShape>&
     return chosen;
 }
 
+// Batch-local scored lists.  In a plain-sum disjunction (every clause score > 0, no MUST_NOT, min_should_match or
+// dismax) a clause that is neither read from a score column nor given a persistent list above — rare, or used once —
+// gets a scored list for this batch only, whatever its df: then every clause of the item is a column or a list and
+// the item runs in the decode-free k_eval_or, which needs fewer registers and no stream cache in shared memory.
+// Same layout and values as a persistent list (k_build_columns<4>); they live in the batch's slab, are freed with it
+// and never enter the list arena or its LRU.  They are taken smallest first within local_list_budget_floats; a clause
+// over the budget stays a block stream and its items stay on the stream variant.  RG_CFG_NO_LISTS / RG_CFG_MAXSCORE:
+// none.
+//
+// The budget per batch is a sixteenth of the HBM free when first needed (after the candidate and list arenas, less
+// what the score columns may still take): a batch's slab can be held by two batches in flight and three idle spare
+// slabs, each with 1/8 headroom, so local lists hold at most about a third of that memory.  Recomputed after an
+// upload.  RG_LOCAL_LISTS_KB sets it (tests).
+static uint64_t local_list_budget_floats(rg_engine* e) {
+    if (!e->local_budget_floats) {
+        if (const char* v = getenv("RG_LOCAL_LISTS_KB")) {
+            e->local_budget_floats = std::max<uint64_t>(1, strtoull(v, nullptr, 10) * 1024 / sizeof(float));
+        } else {
+            size_t free_b = 0, total_b = 0;
+            RG_CUDA_CHECK(cudaMemGetInfo(&free_b, &total_b));
+            const uint64_t col_room = e->col_budget_floats > e->col_floats ? (e->col_budget_floats - e->col_floats) * sizeof(float) : 0;
+            const uint64_t avail = free_b > col_room ? free_b - col_room : 0;
+            e->local_budget_floats = std::max<uint64_t>(1, avail / 16 / sizeof(float));
+        }
+    }
+    return e->local_budget_floats;
+}
+
+void choose_local_lists(rg_engine* e, const std::vector<QShape>& shapes, const rg_clause* clauses, float k1,
+                        const std::map<ColKey, uint32_t>& columns, std::map<ColKey, uint32_t>& lists, HostPlan& hp) {
+    if (e->cfg.flags & (RG_CFG_NO_LISTS | RG_CFG_MAXSCORE)) return;
+    uint32_t k1bits;
+    memcpy(&k1bits, &k1, 4);
+    std::map<ColKey, uint64_t> want;  // clause -> list length in floats: a unit of 256 per block and tail
+    for (const QShape& sh : shapes) {
+        if (sh.type != kTypeOr || sh.match_all || sh.clause_idx.size() >= 10 || sh.msm || sh.dismax || !sh.not_idx.empty())
+            continue;
+        for (uint32_t si = 0; si < e->segs.size(); si++) {
+            const Segment& seg = e->segs[si];
+            auto df_of = [&](const rg_clause& c) -> uint64_t {
+                return c.term_id < seg.host_terms.size() ? (uint64_t)seg.host_terms[c.term_id].doc_freq : 0u;
+            };
+            bool pos = true;  // as plan_batch's item_pos
+            for (uint32_t ci : sh.clause_idx)
+                if (df_of(clauses[ci])) pos = pos && scores_positive(seg, clause_weight(clauses[ci]), clauses[ci].cache_id, k1);
+            if (!pos) continue;
+            for (uint32_t ci : sh.clause_idx) {
+                const rg_clause& c = clauses[ci];
+                const uint64_t df = df_of(c);
+                if (!df) continue;
+                const float w = clause_weight(c);
+                uint32_t wbits;
+                memcpy(&wbits, &w, 4);
+                const ColKey key(si, c.term_id, wbits, c.cache_id, k1bits);
+                if ((df * e->or_col_den >= (uint64_t)seg.max_doc && columns.count(key)) || lists.count(key)) continue;
+                // + one unit: stream_refill prefetches the block after a full block, and a list whose item keeps a
+                // block stream (budget) is read by the stream variant
+                want.emplace(key, (uint64_t)(seg.host_terms[c.term_id].n_blocks + 1u) * 256u);
+            }
+        }
+    }
+    if (want.empty()) return;
+    std::vector<std::pair<uint64_t, ColKey>> order;
+    order.reserve(want.size());
+    for (const auto& kv : want) order.emplace_back(kv.second, kv.first);
+    std::sort(order.begin(), order.end());
+    const uint64_t budget = local_list_budget_floats(e);
+    for (const auto& r : order) {
+        const ColKey& key = r.second;
+        const TermHost& th = e->segs[std::get<0>(key)].host_terms[std::get<1>(key)];
+        // sorted by length: once one does not fit, none of the rest does.  ItemClause.flags carries the reference in
+        // 16 bits; the build launch counts units in 31.
+        if (hp.local_floats + r.first > budget || hp.col_refs.size() >= 65536 ||
+            (uint64_t)hp.local_units + th.n_blocks + 1u > 0x7fffffffu)
+            break;
+        lists[key] = (uint32_t)hp.col_refs.size();
+        hp.local_refs.emplace_back((uint32_t)hp.col_refs.size(), hp.local_floats);
+        hp.col_refs.push_back(ColRef{nullptr, nullptr, nullptr, nullptr, 1.0f, 1.0f});
+        ColumnJob job{};
+        job.seg = std::get<0>(key);
+        job.term_id = std::get<1>(key);
+        const uint32_t wbits = std::get<2>(key);
+        memcpy(&job.weight, &wbits, 4);
+        job.cache_id = std::get<3>(key);
+        job.dst = reinterpret_cast<void*>((uintptr_t)hp.local_floats);  // rebased in rg_batch_prepare
+        job.unit_begin = hp.local_units;
+        hp.local_jobs.push_back(job);
+        hp.local_units += th.n_blocks + (th.tail_n ? 1u : 0u);
+        hp.local_floats += r.first;
+    }
+}
+
 void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
                 uint32_t n_clauses, uint32_t mode, float k1, HostPlan& hp, PlanTimer& tm, PlanScratch& scratch) {
     const uint32_t n_caches = (uint32_t)(e->h_caches.size() / 256);
@@ -733,11 +838,14 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
     tm.mark("classify");
     const std::map<ColKey, uint32_t> columns = choose_columns(e, shapes, clauses, k1, hp, tm);
     tm.mark("columns");
-    const std::map<ColKey, uint32_t> lists = choose_lists(e, shapes, clauses, k1, columns, hp);
+    std::map<ColKey, uint32_t> lists = choose_lists(e, shapes, clauses, k1, columns, hp);
     tm.mark("lists");
+    choose_local_lists(e, shapes, clauses, k1, columns, lists, hp);
+    tm.mark("local_lists");
     uint32_t k1bits;
     memcpy(&k1bits, &k1, 4);
     const bool no_ms = (e->cfg.flags & RG_CFG_MAXSCORE) == 0;
+    const bool lists_on = (e->cfg.flags & (RG_CFG_NO_LISTS | RG_CFG_MAXSCORE)) == 0;
     // Queries are planned in parallel: contiguous chunks, one HostPlan each, concatenated in query order (item order
     // is collection order, so the result equals the serial plan).
     std::mutex refs_mutex;
@@ -904,6 +1012,9 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
             // DisjunctionMaxWeight::create_scorer (disjunction_max_query.rs:135-155): one scorer in this
             // leaf is that scorer; otherwise the tie breaker rides in a meta clause after the item's
             const bool leaf_dismax = shape.dismax && present.size() > 1;
+            // the decode-free k_eval_or: a plain sum whose every clause is a score column or a scored list
+            bool lean = lists_on && leaf_type == (int)kTypeOr && !use_ms && item_pos && nots.empty() && !shape.msm && !leaf_dismax;
+            for (uint32_t i = clause_begin; lean && i < lp.clauses.size(); i++) lean = (lp.clauses[i].flags & (4u | 128u)) != 0;
             if (leaf_dismax) lp.clauses.push_back(ItemClause{0u, shape.tie, 0u, 8u});
             // ranges of ~range_postings postings, at most max_ranges per (query, leaf): long lists get
             // longer ranges (a range is one warp's sequential job; there are thousands of warps)
@@ -950,6 +1061,9 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
                     lp.ms_ids.push_back(idx);
                     lp.ms_rank.push_back((uint32_t)r * rank_step);
                     lp.max_ms_streams = std::max<uint32_t>(lp.max_ms_streams, n_streams);
+                } else if (lean) {
+                    lp.lean_ids.push_back(idx);
+                    lp.lean_rank.push_back((uint32_t)r * rank_step);
                 } else {
                     lp.or_ids.push_back(idx);
                     lp.or_rank.push_back((uint32_t)r * rank_step);
@@ -985,13 +1099,13 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
         for (auto& ep : errs)
             if (ep) std::rethrow_exception(ep);
         // concatenate in query order: offsets first, then every part is copied by its own thread
-        struct Off { size_t items, clauses, or_ids, ms_ids, and_ids, ro_ids, dpq_ids, groups; };
-        std::vector<Off> off(n_threads + 1, Off{0, 0, 0, 0, 0, 0, 0, 0});
+        struct Off { size_t items, clauses, or_ids, ms_ids, and_ids, ro_ids, dpq_ids, lean_ids, groups; };
+        std::vector<Off> off(n_threads + 1, Off{0, 0, 0, 0, 0, 0, 0, 0, 0});
         for (uint32_t t = 0; t < n_threads; t++) {
             const HostPlan& lp = parts[t];
             off[t + 1] = Off{off[t].items + lp.items.size(), off[t].clauses + lp.clauses.size(), off[t].or_ids + lp.or_ids.size(),
                              off[t].ms_ids + lp.ms_ids.size(), off[t].and_ids + lp.and_ids.size(), off[t].ro_ids + lp.ro_ids.size(),
-                             off[t].dpq_ids + lp.dpq_ids.size(), off[t].groups + lp.group_out.size()};
+                             off[t].dpq_ids + lp.dpq_ids.size(), off[t].lean_ids + lp.lean_ids.size(), off[t].groups + lp.group_out.size()};
             hp.postings += lp.postings;
             hp.algo_bytes += lp.algo_bytes;
             hp.max_or_terms = std::max(hp.max_or_terms, lp.max_or_terms);
@@ -1013,6 +1127,8 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
         hp.and_rank.resize(end.and_ids);
         hp.ro_ids.resize(end.ro_ids);
         hp.dpq_ids.resize(end.dpq_ids);
+        hp.lean_ids.resize(end.lean_ids);
+        hp.lean_rank.resize(end.lean_ids);
         hp.group_out.resize(end.groups);
         ths.clear();
         for (uint32_t t = 0; t < n_threads; t++)
@@ -1034,6 +1150,8 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
                 put_ids(hp.and_ids, o.and_ids, lp.and_ids);
                 put_ids(hp.ro_ids, o.ro_ids, lp.ro_ids);
                 put_ids(hp.dpq_ids, o.dpq_ids, lp.dpq_ids);
+                put_ids(hp.lean_ids, o.lean_ids, lp.lean_ids);
+                std::copy(lp.lean_rank.begin(), lp.lean_rank.end(), hp.lean_rank.begin() + o.lean_ids);
                 std::copy(lp.or_rank.begin(), lp.or_rank.end(), hp.or_rank.begin() + o.or_ids);
                 std::copy(lp.ms_rank.begin(), lp.ms_rank.end(), hp.ms_rank.begin() + o.ms_ids);
                 std::copy(lp.and_rank.begin(), lp.and_rank.end(), hp.and_rank.begin() + o.and_ids);
@@ -1059,6 +1177,7 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
     };
     by_rank(hp.or_ids, hp.or_rank);
     by_rank(hp.ms_ids, hp.ms_rank);
+    by_rank(hp.lean_ids, hp.lean_rank);
     by_rank(hp.and_ids, hp.and_rank);
     // heap groups = contiguous item runs starting at chain-start items
     for (uint32_t i = 0; i < hp.items.size(); i++)
@@ -1121,6 +1240,7 @@ int rg_batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries,
     b->list_floats = hp.list_floats;
     b->col_floats = hp.col_floats;
     b->n_ms = (uint32_t)hp.ms_ids.size();
+    b->n_lean = (uint32_t)hp.lean_ids.size();
     b->max_ms_streams = hp.max_ms_streams;
     for (const ColRef& r : hp.col_refs) b->uses_planes = b->uses_planes || r.hi1 != nullptr;
     b->n_dpq = (uint32_t)hp.dpq_ids.size();
@@ -1160,6 +1280,8 @@ int rg_batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries,
     carve(b->dpq_ids, hp.dpq_ids.size());
     carve(b->ro_ids, hp.ro_ids.size());
     carve(b->col_refs, hp.col_refs.size());
+    carve(b->lean_ids, hp.lean_ids.size());
+    carve(b->local_lists, hp.local_floats / 4);
     carve(b->group_item_begin, hp.group_item_begin.size());
     carve(b->group_out, hp.group_out.size());
     // running top-k scores of every OR work item (theta inheritance along a heap chain); skipped when it would
@@ -1202,12 +1324,15 @@ int rg_batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries,
         span.p = reinterpret_cast<T*>(b->slab.p + reinterpret_cast<size_t>(span.p));
     };
     rebase(b->items); rebase(b->clauses); rebase(b->or_ids); rebase(b->and_ids); rebase(b->ms_ids); rebase(b->dpq_ids); rebase(b->ro_ids); rebase(b->col_refs);
+    rebase(b->lean_ids); rebase(b->local_lists);
     rebase(b->group_item_begin); rebase(b->group_out); rebase(b->item_head); rebase(b->item_matches);
     rebase(b->item_theta); rebase(b->item_topk_n); rebase(b->item_topk); rebase(b->arena_next); rebase(b->dbg); rebase(b->out_hits); rebase(b->out_counts);
     rebase(b->out_total);
     if (p->mode == RG_MODE_SEARCH_PARALLEL) rebase(b->leaf_records);
     b->zero_begin = b->slab.p + zero_off;
     b->zero_bytes = off - zero_off;
+    float* local_base = reinterpret_cast<float*>(b->local_lists.p);
+    for (const auto& r : hp.local_refs) hp.col_refs[r.first].col = local_base + r.second;
     cudaStream_t cs = e->copy_stream;
     up(b->items, hp.items, cs);
     up(b->clauses, hp.clauses, cs);
@@ -1216,6 +1341,7 @@ int rg_batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries,
     up(b->ms_ids, hp.ms_ids, cs);
     up(b->dpq_ids, hp.dpq_ids, cs);
     up(b->ro_ids, hp.ro_ids, cs);
+    up(b->lean_ids, hp.lean_ids, cs);
     up(b->col_refs, hp.col_refs, cs);
     up(b->group_item_begin, hp.group_item_begin, cs);
     up(b->group_out, hp.group_out, cs);
@@ -1223,10 +1349,24 @@ int rg_batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries,
     RG_CUDA_CHECK(cudaEventCreateWithFlags(&b->done, cudaEventDisableTiming));
     for (auto& x : b->ev) RG_CUDA_CHECK(cudaEventCreate(&x));
     RG_CUDA_CHECK(cudaEventRecord(b->uploaded, cs));
+    if (!hp.local_jobs.empty()) {
+        // on the engine stream, ahead of this batch's run; `done` is recorded behind it so that the slab is not handed
+        // to another batch while the build may still write it (rg_batch_destroy of a batch that never ran)
+        for (ColumnJob& j : hp.local_jobs) j.dst = local_base + reinterpret_cast<uintptr_t>(j.dst);
+        uint32_t jb = 0;
+        const ColumnJob* d_jobs = stage_jobs(e, hp.local_jobs, jb);
+        launch_build_lists(st, e->d_segs.p, d_jobs, (uint32_t)hp.local_jobs.size(), hp.local_units, e->d_caches.p, p->k1);
+        RG_CUDA_CHECK(cudaEventRecord(e->list_jobs_done[jb], st));
+        RG_CUDA_CHECK(cudaGetLastError());
+        RG_CUDA_CHECK(cudaEventRecord(b->done, st));
+        b->local_built = true;
+        e->launches++;
+        tm.mark("local_lists_build");
+    }
     b->h2d_bytes = (hp.items.size() * sizeof(WorkItem)) + hp.clauses.size() * sizeof(ItemClause) +
-                   4 * (hp.or_ids.size() + hp.ms_ids.size() + hp.dpq_ids.size() + hp.and_ids.size() + hp.ro_ids.size() + hp.group_item_begin.size() + hp.group_out.size()) +
+                   4 * (hp.or_ids.size() + hp.lean_ids.size() + hp.ms_ids.size() + hp.dpq_ids.size() + hp.and_ids.size() + hp.ro_ids.size() + hp.group_item_begin.size() + hp.group_out.size()) +
                    hp.col_refs.size() * sizeof(ColRef);
-    b->kernels_per_run = (b->n_ms ? 1 : 0) + (b->n_dpq ? 1 : 0) + (b->n_or ? 1 : 0) + (b->n_and ? 1 : 0) + (b->n_ro ? 1 : 0) + (b->n_groups ? 1 : 0) +
+    b->kernels_per_run = (b->n_lean ? 1 : 0) + (b->n_ms ? 1 : 0) + (b->n_dpq ? 1 : 0) + (b->n_or ? 1 : 0) + (b->n_and ? 1 : 0) + (b->n_ro ? 1 : 0) + (b->n_groups ? 1 : 0) +
                          (p->mode == RG_MODE_SEARCH_PARALLEL ? 1 : 0);
     tm.mark("alloc_copy_issue");
     RG_CUDA_CHECK(cudaStreamSynchronize(cs));  // the host vectors go out of scope (a running batch is not waited for)
@@ -1273,6 +1413,8 @@ int rg_batch_run(rg_engine* e, rg_batch* b) {
         has_live = has_live || sg.live.p != nullptr;
         has_other = has_other || sg.has_other_enc;
     }
+    launch_eval_or_lean(st, ep, b->lean_ids.p, b->n_lean, has_live);
+    RG_CUDA_CHECK(cudaGetLastError());
     launch_eval_or_ms(st, ep, b->ms_ids.p, b->n_ms, b->max_ms_streams, has_live, b->uses_planes);
     RG_CUDA_CHECK(cudaGetLastError());
     launch_eval_or(st, ep, b->or_ids.p, b->n_or, b->max_or_terms, has_live, b->or_has_not, b->or_has_msm, b->or_has_dmax,
@@ -1340,7 +1482,7 @@ int rg_batch_fetch(rg_engine* e, rg_batch* b, rg_hit* out_hits, uint32_t* out_co
 void rg_batch_destroy(rg_engine* e, rg_batch* b) {
     if (!b) return;
     // hand the slab back for the next batch — whose plan goes up on the copy stream, so this batch's kernels must be over
-    if (e && b->ran && !b->synced) cudaEventSynchronize(b->done);
+    if (e && (b->ran || b->local_built) && !b->synced) cudaEventSynchronize(b->done);
     if (e && b->slab.p) {
         if (e->spare_slabs.size() < 3) {
             e->spare_slabs.push_back(std::move(b->slab));
@@ -1368,7 +1510,7 @@ int rg_batch_stats(rg_engine* e, rg_batch* b, uint64_t out[8]) {
     out[3] = used;
     out[4] = b->kernels_per_run;
     out[5] = b->h2d_bytes;
-    out[6] = b->n_or + b->n_ms + b->n_dpq;
+    out[6] = b->n_or + b->n_lean + b->n_ms + b->n_dpq;
     out[7] = b->n_and + b->n_ro;
     return RG_OK;
     RG_CATCH
@@ -1403,6 +1545,7 @@ int rg_batch_debug(rg_engine* e, rg_batch* b, uint64_t out[16]) {
         RG_CUDA_CHECK(cudaStreamSynchronize(e->stream));
         RG_CUDA_CHECK(cudaMemcpy(out, b->dbg.p, 16 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
     }
+    out[14] = b->n_lean;
     return RG_OK;
     RG_CATCH
 }

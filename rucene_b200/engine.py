@@ -147,6 +147,7 @@ class Batch:
                  "stream_postings", "column_gathers", "refills", "candidates", "steps_scanned", "windows_cut",
                  "windows_scored", "docs_scored"]
         d = {n: int(out[i]) for i, n in enumerate(names)}
+        d["decode_free_items"] = int(out[14])   # the planner's routing (no RG_CFG_STATS needed)
         d["and_touched_bytes"] = int(out[15])   # always counted by k_eval_and (no RG_CFG_STATS needed)
         return d
 
