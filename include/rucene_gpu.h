@@ -55,7 +55,8 @@ extern "C" {
 /* Environment variables read by the library (diagnostics / tuning sweeps; none is needed in production):
  * RG_PLAN_TIMING=1 prints where rg_batch_prepare's host time goes; RG_OR_COL_DEN=n reads a disjunction clause from its
  * score column when df >= max_doc/n (default 8); RG_MAX_RANGES=n caps the docid ranges per (query, leaf) (default 256);
- * RG_LIST_ARENA_KB=n sizes the scored-list arena (default: a sixth of the free HBM, at most 24 GiB). */
+ * RG_LIST_ARENA_KB=n sizes the scored-list arena (default: a sixth of the free HBM, at most 24 GiB); RG_COLUMN_SWEEP=1
+ * makes the decode-free k_eval_or read every score-column cell (no block-maximum bound; A/B runs). */
 
 typedef struct rg_engine rg_engine;
 typedef struct rg_batch rg_batch;
@@ -213,6 +214,9 @@ int rg_batch_stats(rg_engine* e, rg_batch* b, uint64_t out[8]);
  * the bit-sliced bound, [3]=windows before any theta, [4]=docids only counted (between windows), [5]=stream postings
  * visited, [6]=column gathers, [7]=block refills, [8]=candidates, [9]=32-doc steps scanned for candidates,
  * [10]=windows cut by a sparse stream's cache end, [11]=windows with a non-empty scoring set, [12]=docs scored.
+ * [13]=whole windows of the decode-free k_eval_or in which only score columns have postings: low 32 bits = those
+ * counted from the columns' presence bitmaps because their block maxima cannot beat theta, high 32 bits = those whose
+ * cells were read (one atomic per such window).
  * Always counted (no flag needed): [14]=work items the planner sent to the decode-free k_eval_or (every clause a
  * score column or a scored list; known from rg_batch_prepare on), [15]=bytes the conjunction kernel (k_eval_and) asked for in the last run —
  * decoded block parts + 12 B of tables per block, 4 B per skip probe and column gather, 1 norm byte per scored

@@ -745,6 +745,7 @@ int rg_engine_create(const rg_config* cfg, rg_engine** out) {
     e->range_postings_set = e->cfg.range_postings != 0;  // else the planner picks per batch (plan_batch)
     if (e->cfg.range_postings == 0) e->cfg.range_postings = 1u << 15;
     if (const char* v = getenv("RG_OR_COL_DEN")) e->or_col_den = std::max(1, atoi(v));  // tuning knob (bench sweeps)
+    if (const char* v = getenv("RG_COLUMN_SWEEP")) e->column_sweep = atoi(v) != 0;      // A/B knob
     *out = e.release();
     return RG_OK;
     RG_CATCH

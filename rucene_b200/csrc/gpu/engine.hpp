@@ -75,6 +75,9 @@ struct ColRef {
     const uint32_t* hi1;  // plane "tf-norm factor above tau1" of the term for the clause's norm cache (null: none)
     const uint32_t* hi2;  // plane "... above tau2" (a subset of hi1)
     float tau1, tau2;
+    // score column: per kColBlk docids its largest cell, as uint bits (cells are +0.0f or positive, so uint order is
+    // float order); the decode-free k_eval_or bounds a window's column sums with it.  Null: every cell is read
+    const uint32_t* bmax;
 };
 
 // BM25's tf-norm factor f/(f+norm) of most postings is far below 1 (f = 1 in an average-length doc gives 0.45; where
@@ -105,6 +108,7 @@ struct ColEntry {
     float* col = nullptr;  // len floats: its own cudaMalloc (score column) or a piece of the engine's list arena
     bool in_arena = false;
     const uint32_t* bits = nullptr;
+    uint32_t* bmax = nullptr;  // score column: its block-maximum table, in the same allocation (counted in len)
     uint64_t len = 0;
     uint64_t last_use = 0;
     ~ColEntry() {
@@ -198,6 +202,8 @@ struct ColumnJob {
 };
 void launch_build_columns(cudaStream_t st, const SegDev* segs, const ColumnJob* jobs, uint32_t n_jobs,
                           uint32_t n_units, const float* caches, float k1);
+// bmax[b] = the largest of col[b * kColBlk, (b + 1) * kColBlk) as uint bits, b < n_blk
+void launch_col_block_max(cudaStream_t st, const float* col, uint32_t* bmax, uint32_t n_blk);
 // scored posting lists: job.dst = uint4[units * 64], unit = block or vint tail of the job's term
 void launch_build_lists(cudaStream_t st, const SegDev* segs, const ColumnJob* jobs, uint32_t n_jobs, uint32_t n_units,
                         const float* caches, float k1);
@@ -293,6 +299,7 @@ struct rg_engine {
     // (scored list) for df >= max_doc / or_col_den; measured on C4 (one H100 at 400 W, 256 ranges per leaf):
     // 1/4 641 ms, 1/8 627, 1/16 669 per step
     uint64_t or_col_den = 8;
+    bool column_sweep = false;  // RG_COLUMN_SWEEP=1: the decode-free k_eval_or reads every column cell (no block-max bound)
     bool range_postings_set = false;  // rg_config.range_postings was given (else the planner chooses per batch)
     uint64_t generation = 1;            // bumped by rg_segment_upload / rg_norm_cache_set (stale-batch check)
     std::vector<uint8_t> cache_nonneg;  // per norm cache: every entry >= 0 (MaxScore bound needs it)

@@ -266,8 +266,14 @@ constexpr int kNewcW = 64;
 
 struct WTerm {
     const int32_t* blk_last;
-    const BlockDesc* blk_desc;
-    const float* cache;
+    union {
+        const BlockDesc* blk_desc;
+        const uint32_t* col_bmax;  // score column (LEAN): ColRef::bmax, largest cell per kColBlk docids (null: none)
+    };
+    union {
+        const float* cache;
+        const uint32_t* col_bits;  // score column (LEAN): the term's presence bitmap (ColRef::bits)
+    };
     uint32_t nb;        // full blocks; decode-free variant (LEAN): units of the scored list, full blocks + the tail if any
     uint32_t cur;       // next block to decode (nb = vint tail, nb+1 = exhausted); LEAN: the cursor's unit, nb = exhausted
     uint32_t n;         // valid entries in the stream cache
@@ -276,7 +282,10 @@ struct WTerm {
     float w1;           // weight * (k1 + 1)
     uint32_t is_not;    // MUST_NOT clause: its postings exclude docs (search/scorer/req_not_scorer.rs)
     uint32_t is_col;    // score column: blk_last is really a const float* indexed by docid (see k_build_columns)
-    const uint4* pre;   // scored posting list (k_build_columns<4>): 1 KB per block = 128 docids + 128 f32 scores; null = decode
+    union {
+        const uint4* pre;   // scored posting list (k_build_columns<4>): 1 KB per block = 128 docids + 128 f32 scores; null = decode
+        unsigned long long* col_dbg;  // score column (LEAN): EvalParams::dbg (RG_CFG_STATS counters, else null)
+    };
 };
 
 // One posting of a clause lands on window slot idx.  SHOULD clause: clause-order f32 add, first

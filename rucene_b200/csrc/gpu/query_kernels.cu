@@ -130,12 +130,53 @@ __device__ __forceinline__ void count_and_max(const uint4 o, int g, int lane, co
 // memory is neither read nor written.  Returns 0xffffffff when some doc beats theta (the caller then runs the general
 // path to scan the window), else this lane's number of matches.  Not inlined: its 24 live float registers must not weigh on the
 // register allocation of the stream loops.
-template <bool LIVE>
+// BOUND (decode-free variant: windows are 32-aligned, every column carries col_bits and, unless RG_COLUMN_SWEEP, col_bmax):
+// first C = the round-up sum over the columns of their largest cell in the kColBlk-blocks of the window.  If
+// C <= theta' = theta * (1 - 2^-17) (rounded down), no doc of the window can beat theta and its matches are the bits of the
+// columns' ORed presence bitmaps: no cell is read.  Exactness: a doc's score S_f is the round-to-nearest f32 sum, in
+// clause order from +0.0f, of n <= kMaxTerms positive column cells, so with u = 2^-24, S_f <= S (1 + u)^(n-1) for their
+// exact sum S, and S <= C (each cell is at most its block maximum, round-up adds only grow).  Hence
+// S_f <= (1 + 2^-20) C <= (1 + 2^-20)(1 - 2^-17) theta < theta: the window holds no candidate, and its matches are the
+// docs with a posting, i.e. a non-zero sum (every cell of a posting is > 0).  theta = 0 (heap still open) never clears.
+template <bool LIVE, bool BOUND = false>
 __device__ __noinline__ uint32_t columns_only_window(const WTerm* term, uint32_t active, const uint64_t* __restrict__ live,
                                                      int win0, int hi, float te, int lane) {
     uint32_t c = 0;
     float mx = 0.0f;
     const int win1 = win0 + kWw;
+    if (BOUND) {
+        const int b0 = win0 / kColBlk;
+        uint32_t m = 0;
+        bool ok = true;
+        if ((active >> lane) & 1u) {
+            const uint32_t* bm = term[lane].col_bmax;
+            ok = bm != nullptr;
+            if (ok) {
+#pragma unroll
+                for (int j = 0; j <= kWw / kColBlk; j++)  // a 32-aligned window touches at most kWw / kColBlk + 1 blocks
+                    m = max(m, b0 + j <= (win1 - 1) / kColBlk ? __ldg(bm + b0 + j) : 0u);
+            }
+        }
+        bool clear = false;
+        if (__all_sync(0xffffffffu, ok)) {  // (no table: RG_COLUMN_SWEEP)
+            float c_ub = __uint_as_float(m);  // the butterfly leaves the same sum in every lane (a + b == b + a)
+#pragma unroll
+            for (int o = 16; o; o >>= 1) c_ub = __fadd_ru(c_ub, __shfl_xor_sync(0xffffffffu, c_ub, o));
+            clear = c_ub <= __fmul_rd(te, 0.99999237060546875f);  // 1 - 2^-17
+        }
+        unsigned long long* dbg = term[__ffs(active) - 1].col_dbg;
+        if (dbg && lane == 0) atomicAdd(dbg + 13, clear ? 1ull : 1ull << 32);
+        if (clear) {
+            if (lane < kWw / 32) {
+                const int d0 = win0 + lane * 32;
+                uint32_t w = 0;
+                for (uint32_t a = active; a; a &= a - 1) w |= __ldg(term[__ffs(a) - 1].col_bits + (d0 >> 5));
+                if (LIVE && live) w &= (uint32_t)(live[d0 >> 6] >> (d0 & 32));  // d0 % 32 == 0
+                c = __popc(w);
+            }
+            return c;
+        }
+    }
 #pragma unroll
     for (int h = 0; h < kWw / 128; h += 3) {
         float4 s3[3];
@@ -248,8 +289,8 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
         const ItemClause c = p.clauses[it.clause_begin + lane];
         WTerm& tc = sh.term[lane];
         tc.blk_last = reinterpret_cast<const int32_t*>(p.cols[c.term_id].col);
-        tc.blk_desc = nullptr;
-        tc.cache = nullptr;
+        tc.col_bmax = LEAN && p.cols[c.term_id].bits ? p.cols[c.term_id].bmax : nullptr;
+        tc.col_bits = LEAN ? p.cols[c.term_id].bits : nullptr;
         tc.nb = 0;
         tc.cur = 1;  // > nb: exhausted as a stream
         tc.n = 0;
@@ -258,7 +299,7 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
         tc.w1 = 0.0f;
         tc.is_not = 0;
         tc.is_col = (c.flags & 64u) ? 2 : 1;  // 2: every docid present (MatchAllDocsQuery), cells all 0
-        tc.pre = nullptr;
+        tc.col_dbg = LEAN ? p.dbg : nullptr;
     } else if (lane < T) {
         const ItemClause c = p.clauses[it.clause_begin + lane];
         const TermDev td = seg.terms[c.term_id];
@@ -301,8 +342,8 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
         }
     }
     // a column clause has a (potential) posting at every docid: windows become contiguous and
-    // 4-aligned (16-byte column loads) from the start of the range
-    if (lane < T && sh.term[lane].is_col && lo < hi) nd = lo & ~3;
+    // 4-aligned (16-byte column loads) from the start of the range; LEAN: 32-aligned (whole bitmap words)
+    if (lane < T && sh.term[lane].is_col && lo < hi) nd = lo & (LEAN ? ~31 : ~3);
     int w0 = __reduce_min_sync(0xffffffffu, nd);
 
     WEmit em;
@@ -346,7 +387,7 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
         if (POS && active && !__any_sync(0xffffffffu, my_stream && nd < win1) && win1 - win0 == kWw && win0 >= lo) {
             // Only score columns have postings in this (whole) window: see columns_only_window.  Only if a doc beats
             // theta (rare) the general path below redoes the window to scan it.
-            const uint32_t cnt = columns_only_window<LIVE>(sh.term, active, seg.live, win0, hi, te, lane);
+            const uint32_t cnt = columns_only_window<LIVE, LEAN>(sh.term, active, seg.live, win0, hi, te, lane);
             if (cnt != 0xffffffffu) {
                 my_matches += cnt;
                 if ((active >> lane) & 1u) nd = win1 < hi ? win1 : kNoMoreDocs;
@@ -1128,6 +1169,19 @@ void launch_build_columns(cudaStream_t st, const SegDev* segs, const ColumnJob* 
     if (!n_jobs || !n_units) return;
     k_build_columns<0><<<(n_units + kColWarps - 1) / kColWarps, kColWarps * 32, 0, st>>>(segs, jobs, n_jobs, n_units,
                                                                                          caches, k1, nullptr, 0);
+}
+// One warp per table entry: one coalesced float4 per lane, then a warp max.
+__global__ void __launch_bounds__(256) k_col_block_max(const float* __restrict__ col, uint32_t* __restrict__ bmax, uint32_t n_blk) {
+    static_assert(kColBlk == 128, "one float4 per lane");
+    const uint32_t b = blockIdx.x * 8 + (threadIdx.x >> 5);
+    if (b >= n_blk) return;
+    const uint4 v = __ldg(reinterpret_cast<const uint4*>(col + (size_t)b * kColBlk) + lane_id());
+    const uint32_t m = __reduce_max_sync(0xffffffffu, max(max(v.x, v.y), max(v.z, v.w)));
+    if (lane_id() == 0) bmax[b] = m;
+}
+void launch_col_block_max(cudaStream_t st, const float* col, uint32_t* bmax, uint32_t n_blk) {
+    if (!n_blk) return;
+    k_col_block_max<<<(n_blk + 7) / 8, 256, 0, st>>>(col, bmax, n_blk);
 }
 void launch_build_lists(cudaStream_t st, const SegDev* segs, const ColumnJob* jobs, uint32_t n_jobs, uint32_t n_units,
                         const float* caches, float k1) {

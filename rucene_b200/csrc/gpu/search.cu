@@ -487,7 +487,7 @@ std::map<ColKey, uint32_t> choose_columns(rg_engine* e, const std::vector<QShape
     auto add_ref = [&](const ColKey& key, const std::shared_ptr<ColEntry>& ent) {
         ent->last_use = ++e->col_tick;
         chosen[key] = (uint32_t)hp.col_refs.size();
-        ColRef ref{ent->col, ent->bits, nullptr, nullptr, 1.0f, 1.0f};
+        ColRef ref{ent->col, ent->bits, nullptr, nullptr, 1.0f, 1.0f, e->column_sweep ? nullptr : ent->bmax};
         if (std::get<1>(key) != kMatchAllTerm) tf_planes_of(e, std::get<0>(key), std::get<1>(key), std::get<3>(key), k1, ref);
         hp.col_refs.push_back(ref);
         hp.cols.push_back(ent);
@@ -507,6 +507,7 @@ std::map<ColKey, uint32_t> choose_columns(rg_engine* e, const std::vector<QShape
     std::sort(to_build.begin(), to_build.end(), [](const auto& x, const auto& y) { return x.first != y.first ? x.first > y.first : x.second < y.second; });
     tm.mark("col_cached");
     std::vector<ColumnJob> jobs;
+    std::vector<std::shared_ptr<ColEntry>> built;
     uint32_t n_units = 0;
     cudaStream_t st = e->stream;
     if (any_match_all) {
@@ -533,7 +534,9 @@ std::map<ColKey, uint32_t> choose_columns(rg_engine* e, const std::vector<QShape
     for (const auto& r : to_build) {
         if (hp.col_refs.size() >= 4096) break;
         const Segment& seg = e->segs[std::get<0>(r.second)];
-        const uint64_t len = ((uint64_t)seg.max_doc + 1024 + 3) & ~3ull;  // windows read past max_doc
+        // windows read past max_doc; the block-maximum table follows the cells
+        const uint64_t col_len = ((uint64_t)seg.max_doc + 1024 + kColBlk - 1) / kColBlk * kColBlk;
+        const uint64_t len = col_len + ((col_len / kColBlk + 3) & ~3ull);
         if (!make_room(e, len)) break;
         auto ent = std::make_shared<ColEntry>();
         ent->key = r.second;
@@ -545,6 +548,8 @@ std::map<ColKey, uint32_t> choose_columns(rg_engine* e, const std::vector<QShape
         }
         const TermHost& th = seg.host_terms[std::get<1>(r.second)];
         ent->bits = seg.bitmaps.p + (size_t)seg.bitmap_slot[std::get<1>(r.second)] * seg.bitmap_words;
+        ent->bmax = reinterpret_cast<uint32_t*>(ent->col + col_len);
+        built.push_back(ent);
         RG_CUDA_CHECK(cudaMemsetAsync(ent->col, 0, len * sizeof(float), st));
         ColumnJob job{};
         job.seg = std::get<0>(r.second);
@@ -570,6 +575,11 @@ std::map<ColKey, uint32_t> choose_columns(rg_engine* e, const std::vector<QShape
         RG_CUDA_CHECK(cudaGetLastError());
         RG_CUDA_CHECK(cudaEventRecord(e->list_jobs_done[jb], st));
         e->launches++;
+        for (const auto& ent : built) {
+            launch_col_block_max(st, ent->col, ent->bmax, (uint32_t)((reinterpret_cast<float*>(ent->bmax) - ent->col) / kColBlk));
+            RG_CUDA_CHECK(cudaGetLastError());
+            e->launches++;
+        }
         hp.n_cols_built = (uint32_t)jobs.size();
     }
     return chosen;

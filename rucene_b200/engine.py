@@ -147,6 +147,8 @@ class Batch:
                  "stream_postings", "column_gathers", "refills", "candidates", "steps_scanned", "windows_cut",
                  "windows_scored", "docs_scored"]
         d = {n: int(out[i]) for i, n in enumerate(names)}
+        d["column_windows_from_bitmaps"] = int(out[13]) & 0xffffffff   # decode-free k_eval_or: no column cell read
+        d["column_windows_swept"] = int(out[13]) >> 32                 # ... every column cell of the window read
         d["decode_free_items"] = int(out[14])   # the planner's routing (no RG_CFG_STATS needed)
         d["and_touched_bytes"] = int(out[15])   # always counted by k_eval_and (no RG_CFG_STATS needed)
         return d
