@@ -149,7 +149,8 @@ int rg_engine_column_stats(rg_engine* e, uint64_t out[4]);
 int rg_engine_list_stats(rg_engine* e, uint64_t out[4]);
 /* Number of this library's kernels launched so far (bench.py's gpu_launches). */
 uint64_t rg_engine_launch_count(rg_engine* e);
-/* Device-side timing of the last rg_batch_run / rg_blockset_decode, CUDA events on the launch
+/* Device-side timing of the last rg_batch_run / rg_blockset_decode ("run", "eval", "replay", "decode") or
+ * rg_batch_rescore / rg_rescore_hits ("rescore": waits for that launch), CUDA events on the launch
  * stream.  Returns milliseconds, <0 if nothing was timed. */
 float rg_engine_last_kernel_ms(rg_engine* e, const char* which);
 
@@ -224,6 +225,48 @@ int rg_batch_stats(rg_engine* e, rg_batch* b, uint64_t out[8]);
 int rg_batch_debug(rg_engine* e, rg_batch* b, uint64_t out[16]);
 /* Score columns the planner chose for this batch (see RG_CFG_*): how many, and their bytes in HBM. */
 int rg_batch_columns(rg_engine* e, rg_batch* b, uint32_t* n_columns, uint64_t* bytes);
+
+/* ---------------------------------------------------------------- rescoring ------- */
+/* QueryRescorer::rescore (search/scorer/rescorer.rs:130-607) for score TopDocs: the first window_size hits of a
+ * row are sorted by docid, scored by a second query (advance() per hit, one scorer per leaf; a hit matches iff the
+ * scorer lands on it), combined as mode(score * query_weight, new * rescore_weight) where matched and
+ * score * query_weight where not, and sorted again by (score desc, docid asc); every hit after the window gets
+ * score * query_weight and keeps its place.  total_hits is unchanged; a row with total_hits == 0 or no hits is left
+ * as it is.  Live docs are not consulted (advance does not).  Accepted rescoring queries: every shape
+ * rg_batch_prepare accepts, except the ones the reference scores through a DisiPriorityQueue, whose f32 summation
+ * order depends on the heap's history: a pure SHOULD BooleanQuery of >= 10 clauses with min_should_match <= 1 and
+ * a DisjunctionMaxQuery of >= 10 disjuncts give RG_EUNSUPPORTED.  Pure SHOULD queries with min_should_match > 1
+ * are accepted up to 32 clauses; advance() never counts clauses, so min_should_match plays no part in rescoring —
+ * except beside MUST_NOT clauses: ReqNotScorer leaves an excluded hit with next(), which does count them, so whether
+ * a later hit matches depends on that walk, and such a query gives RG_EUNSUPPORTED too. */
+#define RG_RESCORE_AVG 0 /* RescoreMode, rescorer.rs:96-115: (a + b) / 2 */
+#define RG_RESCORE_MAX 1 /* max(a, b) */
+#define RG_RESCORE_MIN 2 /* min(a, b) */
+#define RG_RESCORE_TOTAL 3 /* a + b */
+#define RG_RESCORE_MULTIPLY 4 /* a * b */
+typedef struct {            /* RescoreRequest, rescorer.rs:67-94 */
+    uint32_t window_size;
+    float query_weight;
+    float rescore_weight;
+    uint32_t mode;          /* RG_RESCORE_* */
+    float k1;               /* BM25 k1 of the rescoring query's similarity */
+    uint32_t reserved;      /* 0 */
+} rg_rescore_params;
+
+/* After rg_batch_run and before rg_batch_fetch: rescore query i's TopDocs with queries[i] (n_queries == the
+ * batch's).  Queued on the engine stream; rg_batch_fetch returns the rescored rows.  Calling it twice applies it
+ * twice, as calling Rescorer::rescore twice would.  In RG_MODE_SEARCH_PARALLEL the rows are the merged rows
+ * rg_batch_fetch returns.  Sharded runs are not covered (their hits span engines).  RG_EINVAL: the batch has not
+ * run or is stale, a count mismatch, mode out of range or reserved != 0.  On any error the rows are untouched.
+ * rg_engine_last_kernel_ms(e, "rescore") times the last k_rescore launch. */
+int rg_batch_rescore(rg_engine* e, rg_batch* b, const rg_query* queries, uint32_t n_queries,
+                     const rg_clause* clauses, uint32_t n_clauses, const rg_rescore_params* p);
+/* The same over caller-held TopDocs (host arrays, rows of stride k <= 1024, rewritten in place):
+ * Rescorer::rescore(searcher, &req, &mut top_docs) for hits that came from anywhere, e.g. the CPU searcher's answer
+ * to a query the engine does not accelerate.  Synchronous.  A hit whose docid is in no leaf is RG_EINVAL. */
+int rg_rescore_hits(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                    uint32_t n_clauses, const rg_rescore_params* p, uint32_t k, rg_hit* hits,
+                    const uint32_t* counts, const uint64_t* total_hits);
 
 /* Sharded mode (one segment per GPU).  After rg_batch_run with RG_MODE_SEARCH_PARALLEL the
  * per-query leaf record {uint32 n; uint32 pad; uint64 total_hits; rg_hit heap[k]} (heap-array

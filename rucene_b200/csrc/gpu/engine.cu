@@ -742,6 +742,7 @@ int rg_engine_create(const rg_config* cfg, rg_engine** out) {
     RG_CUDA_CHECK(cudaEventCreate(&e->ev1));
     RG_CUDA_CHECK(cudaEventCreate(&e->ev2));
     RG_CUDA_CHECK(cudaEventCreate(&e->ev3));
+    for (auto& ev : e->rescore_ev) RG_CUDA_CHECK(cudaEventCreate(&ev));
     e->range_postings_set = e->cfg.range_postings != 0;  // else the planner picks per batch (plan_batch)
     if (e->cfg.range_postings == 0) e->cfg.range_postings = 1u << 15;
     if (const char* v = getenv("RG_OR_COL_DEN")) e->or_col_den = std::max(1, atoi(v));  // tuning knob (bench sweeps)
@@ -759,6 +760,8 @@ void rg_engine_destroy(rg_engine* e) {
     if (e->ev1) cudaEventDestroy(e->ev1);
     if (e->ev2) cudaEventDestroy(e->ev2);
     if (e->ev3) cudaEventDestroy(e->ev3);
+    for (auto& ev : e->rescore_ev)
+        if (ev) cudaEventDestroy(ev);
     for (auto& ev : e->list_jobs_done)
         if (ev) cudaEventDestroy(ev);
     if (e->copy_stream) cudaStreamDestroy(e->copy_stream);
@@ -814,6 +817,14 @@ float rg_engine_last_kernel_ms(rg_engine* e, const char* which) {
     if (w == "eval") return e->last_eval_ms;
     if (w == "replay") return e->last_replay_ms;
     if (w == "run") return e->last_run_ms;
+    if (w == "rescore") {
+        if (e->rescore_timed && cudaEventSynchronize(e->rescore_ev[1]) == cudaSuccess) {
+            cudaEventElapsedTime(&e->last_rescore_ms, e->rescore_ev[0], e->rescore_ev[1]);
+            e->rescore_timed = false;
+        }
+        cudaGetLastError();
+        return e->last_rescore_ms;
+    }
     return -1.f;
 }
 

@@ -229,6 +229,40 @@ void launch_eval_or_ms(cudaStream_t st, const EvalParams& p, const uint32_t* ite
 void launch_eval_and(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n, bool req_opt,
                      bool has_other_enc);
 
+// rescore.cu: QueryRescorer over TopDocs rows in HBM.  The rescoring query's scorer per (query, leaf), as
+// BooleanWeight::create_scorer builds it; its clauses are ItemClauses (weight = the clause's scoring weight, flags
+// bit0 MUST_NOT, bit1 optional side of a ReqOptScorer), required ones first (conjunctions in cost order), then the
+// optional ones, then the MUST_NOT ones, each group in clause order.
+enum : uint8_t {
+    kRsNone = 0,  // create_scorer returned None: nothing matches in this leaf
+    kRsTerm = 1,  // TermScorer (a bare TermQuery, or what BooleanQuery::build / DisjunctionMaxQuery collapse to)
+    kRsSum = 2,   // DisjunctionSumScorer: clause order from 0.0f (min_should_match is not looked at by advance)
+    kRsMax = 3,   // DisjunctionMaxScorer: max + (sum - max) * tie
+    kRsConj = 4,  // ConjunctionScorer (one clause: that clause), ReqOptScorer when n_opt > 0
+    kRsAll = 5,   // MatchAllDocsQuery (only MUST_NOT clauses): every docid, score 0
+};
+struct RescoreLeaf {
+    uint32_t clause_begin;
+    uint8_t kind, n_req, n_opt, n_not;
+    float tie;
+};
+struct RescoreParams {
+    const SegDev* segs;
+    uint32_t n_segs;
+    const RescoreLeaf* leaves;  // [n_queries][n_segs]
+    const ItemClause* clauses;
+    const float* caches;
+    float k1;
+    rg_hit* hits;               // rows of stride k, rewritten in place
+    const uint32_t* counts;
+    const unsigned long long* totals;
+    uint32_t n_queries, k, window, mode;
+    float query_weight, rescore_weight;
+    uint32_t ncap;              // power of two >= min(k, window), >= 32: shared-memory slots per query
+};
+size_t rescore_smem_bytes(uint32_t ncap);
+void launch_rescore(cudaStream_t st, const RescoreParams& p);
+
 struct ReplayParams {
     const rg_hit* cand_arena;
     const uint32_t* item_head;
@@ -311,6 +345,10 @@ struct rg_engine {
     uint64_t launches = 0;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr, ev2 = nullptr, ev3 = nullptr;
     float last_decode_ms = -1.f, last_eval_ms = -1.f, last_replay_ms = -1.f, last_run_ms = -1.f;
+    // the last k_rescore launch, timed on the launch stream; read (and waited for) by rg_engine_last_kernel_ms
+    cudaEvent_t rescore_ev[2] = {nullptr, nullptr};
+    bool rescore_timed = false;
+    float last_rescore_ms = -1.f;
     void sync_tables();  // (re)upload SegDev array and norm caches when dirty
 };
 

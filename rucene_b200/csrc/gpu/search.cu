@@ -81,6 +81,7 @@ struct rg_batch {
     // the run waits for `uploaded`, the fetch waits for `done` on the copy stream; timing events are the batch's own
     cudaEvent_t uploaded = nullptr, done = nullptr, ev[4] = {nullptr, nullptr, nullptr, nullptr};
     bool synced = false;  // the host has waited for `done`
+    DevBuf<uint8_t> rescore_plan;  // the last rg_batch_rescore's plan (read by its k_rescore)
     ~rg_batch() {
         for (cudaEvent_t x : {uploaded, done, ev[0], ev[1], ev[2], ev[3]})
             if (x) cudaEventDestroy(x);
@@ -165,8 +166,11 @@ struct QShape {
 // (= BM25 with weight +0: 0 * (k1+1) * f / (f + norm) = +0 for any finite norm)
 inline float clause_weight(const rg_clause& c) { return c.occur == RG_FILTER ? 0.0f : c.weight; }
 
-// BooleanQuery::build + BooleanWeight::create_scorer wiring for the accelerated shapes.
-QShape classify(const rg_query& q, const rg_clause* clauses, uint32_t n_clauses_total) {
+// BooleanQuery::build + BooleanWeight::create_scorer wiring for the accelerated shapes.  rescore: the shape is a
+// rescoring query (rg_batch_rescore), scored through advance() only: shapes whose scorer is a DisiPriorityQueue are
+// refused (its f32 summation order depends on the heap's history), and a pure SHOULD query with
+// min_should_match > 1 (SimpleQueue at any width) is taken up to kDpqMaxTerms clauses.
+QShape classify(const rg_query& q, const rg_clause* clauses, uint32_t n_clauses_total, bool rescore = false) {
     if ((uint64_t)q.clause_begin + q.n_clauses > n_clauses_total) throw ArgError("query clause range out of bounds");
     QShape s;
     if (q.flags & RG_Q_DISMAX) {
@@ -174,6 +178,8 @@ QShape classify(const rg_query& q, const rg_clause* clauses, uint32_t n_clauses_
         // DisjunctionMaxScorer::new (disjunction_scorer.rs:118-139): SimpleQueue below 10 disjuncts
         if (q.n_clauses == 0) throw ArgError("DisjunctionMaxQuery: sub query should not be empty!");
         if (q.n_clauses > (uint32_t)kDpqMaxTerms) throw Unsupported("more than 32 disjuncts");
+        if (rescore && q.n_clauses > (uint32_t)kMaxTerms)
+            throw Unsupported("rescoring with a DisjunctionMaxQuery of 10 or more disjuncts (DisiPriorityQueue order)");
         s.type = kTypeOr;
         for (uint32_t i = 0; i < q.n_clauses; i++) s.clause_idx.push_back(q.clause_begin + i);
         if (q.n_clauses > 1) {  // a single disjunct is the disjunct itself
@@ -204,8 +210,14 @@ QShape classify(const rg_query& q, const rg_clause* clauses, uint32_t n_clauses_
     const size_t n_all = musts.size() + shoulds.size() + filters.size() + must_nots.size();
     if (n_all > (size_t)kMaxTerms) {
         const bool pure_should = musts.empty() && filters.empty() && must_nots.empty();
-        if (!pure_should || n_all > (size_t)kDpqMaxTerms || msm > 1)
+        if (rescore) {
+            if (!pure_should || n_all > (size_t)kDpqMaxTerms)
+                throw Unsupported("more than 9 clauses (only pure SHOULD disjunctions of up to 32 clauses go wider)");
+            if (msm <= 1)
+                throw Unsupported("rescoring with a disjunction of 10 or more clauses and min_should_match <= 1 (DisiPriorityQueue order)");
+        } else if (!pure_should || n_all > (size_t)kDpqMaxTerms || msm > 1) {
             throw Unsupported("more than 9 clauses (only pure SHOULD disjunctions of up to 32 clauses with min_should_match <= 1 go wider)");
+        }
     }
     // BooleanQuery::create_weight (:96-125): must_weights = the MUST clauses, then the FILTER clauses
     // (needs_scores = false); BooleanWeight::create_scorer treats them alike from there on
@@ -239,8 +251,44 @@ QShape classify(const rg_query& q, const rg_clause* clauses, uint32_t n_clauses_
     // top-level SHOULD side.  Beside a MUST it sits behind ReqOptScorer::score -> advance(), which
     // does not look at it (disjunction_scorer.rs:350-363), so those shapes ignore it above.
     s.msm = msm > 1 ? (uint32_t)msm : 0u;
-    if (s.msm > 15u) throw Unsupported("min_should_match > 15");
+    if (s.msm > 15u && !rescore) throw Unsupported("min_should_match > 15");
     return s;
+}
+
+// BooleanWeight::create_scorer / DisjunctionMaxWeight::create_scorer for one (query, leaf): which clauses of the
+// shape have a scorer in the leaf.  present: the scoring clauses (a conjunction's required ones), a conjunction's
+// stably sorted by cost() = doc_freq (ConjunctionScorer::new, :30); nots: the MUST_NOT clauses (:236-251); opts:
+// the SHOULD clauses beside a MUST (:217-234).  False when the scorer is None: a required clause is absent
+// (:201-206), no clause exists, or fewer SHOULD clauses than min_should_match exist.
+bool resolve_leaf(const QShape& shape, const Segment& seg, const rg_clause* clauses, std::vector<uint32_t>& present,
+                  std::vector<uint32_t>& nots, std::vector<uint32_t>& opts) {
+    present.clear();
+    nots.clear();
+    opts.clear();
+    bool dead = false;
+    for (uint32_t ci : shape.clause_idx) {
+        const uint32_t t = clauses[ci].term_id;
+        const int32_t df = t < seg.host_terms.size() ? seg.host_terms[t].doc_freq : 0;
+        if (df > 0) present.push_back(ci);
+        else if (shape.type != kTypeOr) dead = true;  // create_scorer -> None (:201-206)
+    }
+    if (dead || (present.empty() && !shape.match_all)) return false;
+    if (shape.type == kTypeOr && shape.msm > present.size()) return false;  // nothing can reach msm here
+    for (uint32_t ci : shape.not_idx) {
+        const uint32_t t = clauses[ci].term_id;
+        if (t < seg.host_terms.size() && seg.host_terms[t].doc_freq > 0) nots.push_back(ci);
+    }
+    for (uint32_t ci : shape.opt_idx) {
+        const uint32_t t = clauses[ci].term_id;
+        if (t < seg.host_terms.size() && seg.host_terms[t].doc_freq > 0) opts.push_back(ci);
+    }
+    if (shape.type != kTypeOr) {
+        // ConjunctionScorer::new: stable sort by cost() = doc_freq (:30)
+        std::stable_sort(present.begin(), present.end(), [&](uint32_t a, uint32_t b) {
+            return seg.host_terms[clauses[a].term_id].doc_freq < seg.host_terms[clauses[b].term_id].doc_freq;
+        });
+    }
+    return true;
 }
 
 // Score columns: which (leaf, term, weight, norm cache, k1) clauses of the batch's disjunctions are read
@@ -867,28 +915,10 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
         uint32_t chain_pos = 0;
         for (uint32_t si = 0; si < n_segs; si++) {
             const Segment& seg = e->segs[si];
-            // resolve clauses against this leaf
-            std::vector<uint32_t> present;
-            bool dead = false;
-            for (uint32_t ci : shape.clause_idx) {
-                const uint32_t t = clauses[ci].term_id;
-                const int32_t df = t < seg.host_terms.size() ? seg.host_terms[t].doc_freq : 0;
-                if (df > 0) present.push_back(ci);
-                else if (shape.type != kTypeOr) dead = true;  // create_scorer -> None (:201-206)
-            }
+            // resolve clauses against this leaf: present (conjunctions in cost order), MUST_NOT, optional side
+            std::vector<uint32_t> present, nots, opts;
             const bool new_group = mode == RG_MODE_SEARCH_PARALLEL || !group_open;
-            if (dead || (present.empty() && !shape.match_all)) continue;
-            if (shape.type == kTypeOr && shape.msm > present.size()) continue;  // nothing can reach msm here
-            std::vector<uint32_t> nots;  // MUST_NOT clauses present in this leaf (:236-251)
-            for (uint32_t ci : shape.not_idx) {
-                const uint32_t t = clauses[ci].term_id;
-                if (t < seg.host_terms.size() && seg.host_terms[t].doc_freq > 0) nots.push_back(ci);
-            }
-            std::vector<uint32_t> opts;  // SHOULD clauses present in this leaf (:217-234)
-            for (uint32_t ci : shape.opt_idx) {
-                const uint32_t t = clauses[ci].term_id;
-                if (t < seg.host_terms.size() && seg.host_terms[t].doc_freq > 0) opts.push_back(ci);
-            }
+            if (!resolve_leaf(shape, seg, clauses, present, nots, opts)) continue;
             // no SHOULD scorer in this leaf -> the MUST side alone, no ReqOptScorer (:259-266)
             // ten or more sub-scorers in this leaf: DisjunctionSumScorer / DisjunctionMaxScorer switch to the
             // DisiPriorityQueue (disjunction_scorer.rs:41-45,118-139), whose summation order only k_eval_dpq reproduces
@@ -899,10 +929,6 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
             if (shape.match_all) {
                 cost = total_df = (uint64_t)seg.max_doc;  // AllDocsIterator: every docid of the leaf
             } else if (shape.type != kTypeOr) {
-                // ConjunctionScorer::new: stable sort by cost() = doc_freq (:30)
-                std::stable_sort(present.begin(), present.end(), [&](uint32_t a, uint32_t b) {
-                    return seg.host_terms[clauses[a].term_id].doc_freq < seg.host_terms[clauses[b].term_id].doc_freq;
-                });
                 cost = (uint64_t)seg.host_terms[clauses[present[0]].term_id].doc_freq;
                 const TermHost& lead = seg.host_terms[clauses[present[0]].term_id];
                 bytes = lead.enc_bytes + cost;
@@ -1195,6 +1221,106 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
     hp.group_item_begin.push_back((uint32_t)hp.items.size());
     if (hp.group_item_begin.size() != hp.group_out.size() + 1) throw ArgError("internal: group bookkeeping mismatch");
     tm.mark("order");
+}
+
+// The rescoring query's scorer per (query, leaf) for k_rescore (RescoreLeaf, engine.hpp), from the same shape
+// resolution as the first pass (classify + resolve_leaf).  Plans every query before anything is launched, so a
+// refused shape leaves the rows untouched.
+struct RescorePlan {
+    std::vector<RescoreLeaf> leaves;  // [n_queries][n_segs]
+    std::vector<ItemClause> clauses;
+};
+
+void plan_rescore(const rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                  uint32_t n_clauses, RescorePlan& rp) {
+    const uint32_t n_caches = (uint32_t)(e->h_caches.size() / 256);
+    const uint32_t n_segs = (uint32_t)e->segs.size();
+    rp.leaves.assign((size_t)n_queries * n_segs, RescoreLeaf{0u, kRsNone, 0, 0, 0, 0.0f});
+    rp.clauses.clear();
+    std::vector<uint32_t> present, nots, opts;
+    for (uint32_t qi = 0; qi < n_queries; qi++) {
+        QShape shape = classify(queries[qi], clauses, n_clauses, true);
+        // ReqNotScorer moves past an excluded hit with next(), and a SHOULD disjunction with min_should_match > 1
+        // then skips to the next doc that reaches min_should_match: whether a later hit matches depends on the walk
+        if (shape.msm > 1 && !shape.not_idx.empty())
+            throw Unsupported("rescoring with a min_should_match > 1 disjunction beside MUST_NOT clauses");
+        // advance() never counts clauses (disjunction_scorer.rs:350-364), and BooleanWeight::create_scorer builds the
+        // DisjunctionSumScorer over whatever SHOULD clauses exist in the leaf, however few: min_should_match plays
+        // no part in rescoring
+        shape.msm = 0;
+        for (const auto* idx : {&shape.clause_idx, &shape.opt_idx, &shape.not_idx})
+            for (uint32_t ci : *idx)
+                if (clauses[ci].cache_id >= n_caches) throw ArgError("clause refers to an unset norm cache");
+        // a bare TermQuery, or what BooleanQuery::build / DisjunctionMaxQuery::build collapse to one clause: the
+        // TermScorer itself (a DisjunctionSumScorer would add it to 0.0f)
+        const bool single = shape.type == kTypeOr && !shape.match_all && !shape.dismax && shape.clause_idx.size() == 1 &&
+                            shape.not_idx.empty();
+        for (uint32_t si = 0; si < n_segs; si++) {
+            if (!resolve_leaf(shape, e->segs[si], clauses, present, nots, opts)) continue;
+            RescoreLeaf& L = rp.leaves[(size_t)qi * n_segs + si];
+            L.clause_begin = (uint32_t)rp.clauses.size();
+            if (shape.match_all) L.kind = kRsAll;
+            else if (shape.type != kTypeOr) L.kind = kRsConj;
+            else if (shape.dismax) L.kind = present.size() > 1 ? kRsMax : kRsTerm;  // one scorer: that scorer (:135-155)
+            else L.kind = single ? kRsTerm : kRsSum;
+            L.tie = shape.tie;
+            L.n_req = (uint8_t)present.size();
+            L.n_opt = (uint8_t)opts.size();
+            L.n_not = (uint8_t)nots.size();
+            for (uint32_t ci : present) rp.clauses.push_back(ItemClause{clauses[ci].term_id, clause_weight(clauses[ci]), clauses[ci].cache_id, 0u});
+            for (uint32_t ci : opts) rp.clauses.push_back(ItemClause{clauses[ci].term_id, clauses[ci].weight, clauses[ci].cache_id, 2u});
+            for (uint32_t ci : nots) rp.clauses.push_back(ItemClause{clauses[ci].term_id, 0.0f, clauses[ci].cache_id, 1u});
+        }
+    }
+}
+
+void check_rescore_params(const rg_rescore_params* p) {
+    if (p->mode > RG_RESCORE_MULTIPLY) throw ArgError("rescore mode out of range");
+    if (p->reserved != 0) throw ArgError("rg_rescore_params.reserved must be 0");
+}
+
+// Upload the plan into `buf` and queue k_rescore over device rows of stride k, both on the engine stream, timed by
+// the engine's rescore events.  No host wait: the copy is ordered behind any earlier k_rescore that reads `buf` (a
+// buffer that has to grow is freed by cudaFree, which waits for the device), and a copy from pageable memory returns
+// once the host vectors have been staged.
+void queue_rescore(rg_engine* e, const RescorePlan& rp, DevBuf<uint8_t>& buf, const rg_rescore_params* p,
+                   uint32_t n_queries, uint32_t k, rg_hit* d_hits, const uint32_t* d_counts,
+                   const unsigned long long* d_totals) {
+    cudaStream_t st = e->stream;
+    const size_t leaves_b = (rp.leaves.size() * sizeof(RescoreLeaf) + 255) & ~(size_t)255;
+    const size_t total = leaves_b + std::max<size_t>(1, rp.clauses.size()) * sizeof(ItemClause);
+    if (buf.n < total) buf.alloc(total);
+    if (!rp.leaves.empty())
+        RG_CUDA_CHECK(cudaMemcpyAsync(buf.p, rp.leaves.data(), rp.leaves.size() * sizeof(RescoreLeaf), cudaMemcpyHostToDevice,
+                                      st));
+    if (!rp.clauses.empty())
+        RG_CUDA_CHECK(cudaMemcpyAsync(buf.p + leaves_b, rp.clauses.data(), rp.clauses.size() * sizeof(ItemClause),
+                                      cudaMemcpyHostToDevice, st));
+    RescoreParams rs{};
+    rs.segs = e->d_segs.p;
+    rs.n_segs = (uint32_t)e->segs.size();
+    rs.leaves = reinterpret_cast<const RescoreLeaf*>(buf.p);
+    rs.clauses = reinterpret_cast<const ItemClause*>(buf.p + leaves_b);
+    rs.caches = e->d_caches.p;
+    rs.k1 = p->k1;
+    rs.hits = d_hits;
+    rs.counts = d_counts;
+    rs.totals = d_totals;
+    rs.n_queries = n_queries;
+    rs.k = k;
+    rs.window = p->window_size;
+    rs.mode = p->mode;
+    rs.query_weight = p->query_weight;
+    rs.rescore_weight = p->rescore_weight;
+    uint32_t ncap = 32;
+    while (ncap < std::min(k, p->window_size)) ncap <<= 1;
+    rs.ncap = ncap;
+    RG_CUDA_CHECK(cudaEventRecord(e->rescore_ev[0], st));
+    launch_rescore(st, rs);
+    RG_CUDA_CHECK(cudaGetLastError());
+    RG_CUDA_CHECK(cudaEventRecord(e->rescore_ev[1], st));
+    e->rescore_timed = true;
+    if (n_queries) e->launches++;
 }
 
 template <class T>
@@ -1633,6 +1759,67 @@ int rg_merge_leaf_records(rg_engine* e, const void* dev_records_all, uint32_t n_
     if (!e || !dev_records_all || !out_hits || !out_counts || !out_total_hits) throw ArgError("null argument");
     merge_on_device(e, dev_records_all, n_leaves, n_queries, k);
     return rg_merge_fetch(e, out_hits, out_counts, out_total_hits);
+    RG_CATCH
+}
+
+int rg_batch_rescore(rg_engine* e, rg_batch* b, const rg_query* queries, uint32_t n_queries,
+                     const rg_clause* clauses, uint32_t n_clauses, const rg_rescore_params* p) {
+    RG_TRY
+    if (!e || !b || !p || (n_queries && !queries) || (n_clauses && !clauses)) throw ArgError("null argument");
+    check_rescore_params(p);
+    if (!b->ran) throw ArgError("rg_batch_rescore before rg_batch_run");
+    if (b->generation != e->generation)
+        throw ArgError("stale batch: a segment was uploaded or a norm cache changed after rg_batch_prepare");
+    if (n_queries != b->n_queries) throw ArgError("rg_batch_rescore: n_queries differs from the batch's");
+    RG_CUDA_CHECK(cudaSetDevice(e->device));
+    RescorePlan rp;
+    plan_rescore(e, queries, n_queries, clauses, n_clauses, rp);
+    queue_rescore(e, rp, b->rescore_plan, p, n_queries, b->k, b->out_hits.p, b->out_counts.p, b->out_total.p);
+    RG_CUDA_CHECK(cudaEventRecord(b->done, e->stream));  // rg_batch_fetch waits for the rescored rows
+    b->synced = false;
+    return RG_OK;
+    RG_CATCH
+}
+
+int rg_rescore_hits(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                    uint32_t n_clauses, const rg_rescore_params* p, uint32_t k, rg_hit* hits,
+                    const uint32_t* counts, const uint64_t* total_hits) {
+    RG_TRY
+    if (!e || !p || (n_queries && (!queries || !hits || !counts || !total_hits)) || (n_clauses && !clauses))
+        throw ArgError("null argument");
+    check_rescore_params(p);
+    if (k == 0) throw ArgError("k must be >= 1");
+    if (k > 1024) throw Unsupported("rows of more than 1024 hits are not accelerated");
+    if (e->segs.empty()) throw ArgError("no segment uploaded");
+    for (uint32_t qi = 0; qi < n_queries; qi++) {
+        if (counts[qi] > k) throw ArgError("a row's count exceeds k");
+        for (uint32_t i = 0; i < counts[qi]; i++) {
+            const int32_t d = hits[(size_t)qi * k + i].doc;
+            bool in_leaf = false;
+            for (const Segment& sg : e->segs) in_leaf = in_leaf || (d >= sg.doc_base && d - sg.doc_base < sg.max_doc);
+            if (!in_leaf) throw ArgError("hit docid " + std::to_string(d) + " is in no leaf");
+        }
+    }
+    RG_CUDA_CHECK(cudaSetDevice(e->device));
+    e->sync_tables();
+    RescorePlan rp;
+    plan_rescore(e, queries, n_queries, clauses, n_clauses, rp);
+    if (n_queries == 0) return RG_OK;
+    const size_t hits_b = ((size_t)n_queries * k * sizeof(rg_hit) + 255) & ~(size_t)255;
+    const size_t counts_b = ((size_t)n_queries * 4 + 255) & ~(size_t)255;
+    DevBuf<uint8_t> rows, plan;
+    rows.alloc(hits_b + counts_b + (size_t)n_queries * 8);
+    rg_hit* d_hits = reinterpret_cast<rg_hit*>(rows.p);
+    uint32_t* d_counts = reinterpret_cast<uint32_t*>(rows.p + hits_b);
+    unsigned long long* d_total = reinterpret_cast<unsigned long long*>(rows.p + hits_b + counts_b);
+    cudaStream_t st = e->stream;
+    RG_CUDA_CHECK(cudaMemcpyAsync(d_hits, hits, (size_t)n_queries * k * sizeof(rg_hit), cudaMemcpyHostToDevice, st));
+    RG_CUDA_CHECK(cudaMemcpyAsync(d_counts, counts, (size_t)n_queries * 4, cudaMemcpyHostToDevice, st));
+    RG_CUDA_CHECK(cudaMemcpyAsync(d_total, total_hits, (size_t)n_queries * 8, cudaMemcpyHostToDevice, st));
+    queue_rescore(e, rp, plan, p, n_queries, k, d_hits, d_counts, d_total);
+    RG_CUDA_CHECK(cudaMemcpyAsync(hits, d_hits, (size_t)n_queries * k * sizeof(rg_hit), cudaMemcpyDeviceToHost, st));
+    RG_CUDA_CHECK(cudaStreamSynchronize(st));
+    return RG_OK;
     RG_CATCH
 }
 

@@ -8,8 +8,10 @@
 //   search/collector/top_docs.rs:107-124 TopDocsCollector::new(k) / top_docs()
 //   search/sort_field/collapse_top_docs.rs:22-68,288-326 ScoreDoc / TopDocs
 //   search/similarity/bm25_similarity.rs:45-46,151-177 BM25Similarity, compute_weight
+//   search/scorer/rescorer.rs:67-115,542-556 RescoreRequest, RescoreMode, QueryRescorer::rescore
 // (paths relative to src/core/ of zhihu/rucene).  Header-only; link librucene_gpu.so.
 #pragma once
+#include <algorithm>
 #include <cstdint>
 #include <memory>
 #include <stdexcept>
@@ -100,6 +102,7 @@ public:
     TopDocs(uint64_t total, std::vector<ScoreDoc> docs) : total_hits_(total), score_docs_(std::move(docs)) {}
     uint64_t total_hits() const { return total_hits_; }
     const std::vector<ScoreDoc>& score_docs() const { return score_docs_; }
+    std::vector<ScoreDoc>& score_docs_mut() { return score_docs_; }
 
 private:
     uint64_t total_hits_ = 0;
@@ -187,6 +190,23 @@ public:
 
     rg_engine* engine() { return engine_; }
 
+    // The device side of QueryRescorer::rescore (below): rg_rescore_hits over top_docs as one row
+    void rescore_top_docs(const Query& query, uint32_t window_size, float query_weight, float rescore_weight,
+                          uint32_t mode, TopDocs& top_docs) {
+        std::vector<ScoreDoc>& docs = top_docs.score_docs_mut();
+        if (top_docs.total_hits() == 0 || docs.empty()) return;  // rescorer.rs:548-550
+        std::vector<rg_clause> clauses;
+        rg_query q = compile(query, clauses);
+        std::vector<rg_hit> hits(docs.size());
+        for (size_t i = 0; i < docs.size(); i++) hits[i] = rg_hit{docs[i].doc, docs[i].score};
+        const uint32_t count = (uint32_t)docs.size();
+        const uint64_t total = top_docs.total_hits();
+        rg_rescore_params p{window_size, query_weight, rescore_weight, mode, sim_.k1, 0};
+        check(rg_rescore_hits(engine_, &q, 1, clauses.data(), (uint32_t)clauses.size(), &p, count, hits.data(), &count,
+                              &total));
+        for (size_t i = 0; i < docs.size(); i++) docs[i] = ScoreDoc{hits[i].doc, hits[i].score};
+    }
+
 private:
     void check(int rc) {
         if (rc == RG_OK) return;
@@ -260,6 +280,36 @@ private:
     int32_t max_doc_ = 0;
     size_t stats_ = 0;
     float avgdl_ = 1.0f;
+};
+
+// RescoreMode / RescoreRequest / QueryRescorer (search/scorer/rescorer.rs:67-115,542-556) for score TopDocs:
+// the first window_size hits are rescored by request.query on the GPU and sorted again, the rest are scaled by
+// query_weight.  More than 1024 hits, or a rescoring query outside the accelerated shapes, throws UnsupportedQuery
+// (the caller then uses the CPU rescorer).
+enum class RescoreMode : uint32_t {
+    Avg = RG_RESCORE_AVG,
+    Max = RG_RESCORE_MAX,
+    Min = RG_RESCORE_MIN,
+    Total = RG_RESCORE_TOTAL,
+    Multiply = RG_RESCORE_MULTIPLY,
+};
+
+struct RescoreRequest {
+    QueryPtr query;
+    float query_weight = 1.0f;
+    float rescore_weight = 1.0f;
+    RescoreMode rescore_mode = RescoreMode::Total;
+    size_t window_size = 10;
+};
+
+class QueryRescorer {
+public:
+    void rescore(GpuIndexSearcher& searcher, const RescoreRequest& req, TopDocs& top_docs) const {
+        if (!req.query) throw IllegalArgument("RescoreRequest without a query");
+        const uint32_t window = (uint32_t)std::min<size_t>(req.window_size, 0xffffffffu);
+        searcher.rescore_top_docs(*req.query, window, req.query_weight, req.rescore_weight,
+                                  (uint32_t)req.rescore_mode, top_docs);
+    }
 };
 
 }  // namespace rucene

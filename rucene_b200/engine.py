@@ -17,6 +17,7 @@ Q_DISMAX = 2    # rg_query.flags: DisjunctionMaxQuery; min_should_match = bits o
 MODE_SEARCH, MODE_SEARCH_PARALLEL = 0, 1
 CFG_NO_COLUMNS, CFG_EAGER_COLUMNS, CFG_NO_BITMAPS, CFG_MAXSCORE, CFG_STATS, CFG_TFPLANES, CFG_NO_LISTS = 1, 2, 4, 8, 16, 32, 64   # rg_config.flags (include/rucene_gpu.h)
 NO_MORE_DOCS = 0x7FFFFFFF
+RESCORE_AVG, RESCORE_MAX, RESCORE_MIN, RESCORE_TOTAL, RESCORE_MULTIPLY = 0, 1, 2, 3, 4   # RescoreMode (rg_rescore_params.mode)
 
 TERM_STATE_DTYPE = np.dtype([("doc_freq", "<i4"), ("singleton_doc_id", "<i4"),
                              ("total_term_freq", "<i8"), ("doc_start_fp", "<i8"),
@@ -36,6 +37,11 @@ class Config(C.Structure):
 class SearchParams(C.Structure):
     _fields_ = [("k", C.c_uint32), ("k1", C.c_float), ("mode", C.c_uint32),
                 ("reserved", C.c_uint32)]
+
+
+class RescoreParams(C.Structure):
+    _fields_ = [("window_size", C.c_uint32), ("query_weight", C.c_float), ("rescore_weight", C.c_float),
+                ("mode", C.c_uint32), ("k1", C.c_float), ("reserved", C.c_uint32)]
 
 
 class EngineError(RuntimeError):
@@ -95,6 +101,9 @@ def lib():
     L.rg_merge_leaf_records_device.argtypes = [vp, vp, C.c_uint32, C.c_uint32, C.c_uint32]
     L.rg_merge_fetch.argtypes = [vp, vp, vp, vp]
     L.rg_merge_leaf_records.argtypes = [vp, vp, C.c_uint32, C.c_uint32, C.c_uint32, vp, vp, vp]
+    L.rg_batch_rescore.argtypes = [vp, vp, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(RescoreParams)]
+    L.rg_rescore_hits.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(RescoreParams), C.c_uint32, vp, vp,
+                                  vp]
     L.rg_segment_decode.argtypes = [vp, C.c_uint32, C.c_uint64, C.c_uint64, vp, vp]
     L.rg_forutil_decode.argtypes = [vp, vp, C.c_size_t, vp, C.c_uint32, C.c_int, vp, vp]
     L.rg_blockset_stage.argtypes = [vp, vp, C.c_size_t, vp, C.c_uint32, C.c_int, vp, C.POINTER(vp)]
@@ -331,6 +340,32 @@ class Engine:
         _check(lib().rg_batch_prepare(self.h, _p(q), len(q), _p(c), len(c), C.byref(p), C.byref(h)),
                self.h)
         return Batch(self, h.value, len(q), k)
+
+    # ---- QueryRescorer (rescorer.rs) ----
+    @staticmethod
+    def _rescore_params(window_size, query_weight, rescore_weight, mode, k1):
+        return RescoreParams(min(int(window_size), 0xFFFFFFFF), query_weight, rescore_weight, mode, k1, 0)
+
+    def rescore_batch(self, batch, queries, clauses, window_size, query_weight=1.0, rescore_weight=1.0,
+                      mode=RESCORE_TOTAL, k1=1.2):
+        """rg_batch_rescore: after batch.run(), before batch.fetch(); rescores the batch's rows on the device."""
+        q = np.ascontiguousarray(queries, dtype=QUERY_DTYPE)
+        c = np.ascontiguousarray(clauses, dtype=CLAUSE_DTYPE)
+        p = self._rescore_params(window_size, query_weight, rescore_weight, mode, k1)
+        _check(lib().rg_batch_rescore(self.h, batch.h, _p(q), len(q), _p(c), len(c), C.byref(p)), self.h)
+
+    def rescore_hits(self, queries, clauses, hits, counts, total, window_size, query_weight=1.0, rescore_weight=1.0,
+                     mode=RESCORE_TOTAL, k1=1.2):
+        """rg_rescore_hits over host rows (hits [n, k] of HIT_DTYPE); returns the rescored copy of hits."""
+        q = np.ascontiguousarray(queries, dtype=QUERY_DTYPE)
+        c = np.ascontiguousarray(clauses, dtype=CLAUSE_DTYPE)
+        h = np.array(hits, dtype=HIT_DTYPE, copy=True, order="C").reshape(len(q), -1)
+        n = np.ascontiguousarray(counts, dtype=np.uint32)
+        t = np.ascontiguousarray(total, dtype=np.uint64)
+        p = self._rescore_params(window_size, query_weight, rescore_weight, mode, k1)
+        _check(lib().rg_rescore_hits(self.h, _p(q), len(q), _p(c), len(c), C.byref(p), h.shape[1], _p(h), _p(n),
+                                     _p(t)), self.h)
+        return h
 
     def merge_leaf_records(self, dev_ptr, n_leaves, n_queries, k):
         hits = np.zeros((n_queries, k), HIT_DTYPE)

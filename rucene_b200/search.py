@@ -12,11 +12,13 @@ src/core/ of zhihu/rucene):
     TopDocsCollector     search/collector/top_docs.rs:107-124 TopDocsCollector::new(k) / top_docs()
     TopDocs / ScoreDoc   search/sort_field/collapse_top_docs.rs:22-68,288-326
     IndexSearcher.search search/searcher.rs:238-240,487-525
+    RescoreMode / RescoreRequest / QueryRescorer   search/scorer/rescorer.rs:67-115,130-607
 
 Everything that touches postings runs on the GPU through the C ABI (engine.py); this module only
 does what Query::create_weight does on the host once per query: collection/term statistics from
 the largest segment (searcher.rs:311-351,732-767) and the BM25 weight (bm25_similarity.rs:151-177).
 """
+import enum
 from dataclasses import dataclass, field
 from typing import List, Optional, Sequence
 
@@ -141,6 +143,46 @@ class TopDocs:
 
     def score_docs(self):
         return self._score_docs
+
+
+class RescoreMode(enum.IntEnum):
+    """rescorer.rs:96-115 — how a matched hit's two scores combine (f32)."""
+    Avg = engine.RESCORE_AVG
+    Max = engine.RESCORE_MAX
+    Min = engine.RESCORE_MIN
+    Total = engine.RESCORE_TOTAL
+    Multiply = engine.RESCORE_MULTIPLY
+
+
+@dataclass
+class RescoreRequest:
+    """RescoreRequest::new (rescorer.rs:67-94); rescore_movedout is never read by the reference and is left out."""
+    query: Query
+    query_weight: float = 1.0
+    rescore_weight: float = 1.0
+    mode: RescoreMode = RescoreMode.Total
+    window_size: int = 10
+
+
+class QueryRescorer:
+    """QueryRescorer::rescore (rescorer.rs:130-140) for score TopDocs: the first window_size hits are scored by
+    request.query on the GPU (rg_rescore_hits), combined with their first-pass score and sorted again; the hits
+    after the window are scaled by query_weight.  top_docs is edited in place."""
+
+    def rescore(self, searcher, request: RescoreRequest, top_docs: TopDocs):
+        docs = top_docs.score_docs()
+        if top_docs.total_hits() == 0 or not docs:
+            return
+        q, c = searcher.compile_batch([request.query])
+        hits = np.zeros((1, len(docs)), engine.HIT_DTYPE)
+        hits[0]["doc"] = [d.doc for d in docs]
+        hits[0]["score"] = np.array([d.score for d in docs], np.float32)
+        out = searcher.engine.rescore_hits(q, c, hits, [len(docs)], [top_docs.total_hits()], request.window_size,
+                                           request.query_weight, request.rescore_weight, int(request.mode),
+                                           k1=searcher.similarity.k1)
+        for i, h in enumerate(out[0]):
+            docs[i].doc = int(h["doc"])
+            docs[i].score = float(h["score"])
 
 
 class TopDocsCollector:
@@ -312,9 +354,22 @@ class GpuIndexSearcher:
         return (np.array(qs, dtype=engine.QUERY_DTYPE).reshape(-1),
                 np.array(clauses, dtype=engine.CLAUSE_DTYPE).reshape(-1))
 
-    def search_batch(self, queries, k, mode=engine.MODE_SEARCH):
+    def search_batch(self, queries, k, mode=engine.MODE_SEARCH, rescore=None):
+        """rescore: (rescoring queries, RescoreRequest) — one rescoring query per query, the request's weights,
+        mode and window for all: QueryRescorer::rescore on every row on the device before the rows are fetched."""
         q, c = self.compile_batch(queries)
-        return self.engine.search_batch(q, c, k, k1=self.similarity.k1, mode=mode)
+        if rescore is None:
+            return self.engine.search_batch(q, c, k, k1=self.similarity.k1, mode=mode)
+        rescore_queries, req = rescore
+        rq, rc = self.compile_batch(rescore_queries)
+        batch = self.engine.prepare(q, c, k, k1=self.similarity.k1, mode=mode)
+        try:
+            batch.run()
+            self.engine.rescore_batch(batch, rq, rc, req.window_size, req.query_weight, req.rescore_weight,
+                                      int(req.mode), k1=self.similarity.k1)
+            return batch.fetch()
+        finally:
+            batch.close()
 
     def search(self, query, collector: TopDocsCollector):
         """IndexSearcher::search(&query, &mut collector)."""
