@@ -226,6 +226,45 @@ int rg_batch_debug(rg_engine* e, rg_batch* b, uint64_t out[16]);
 /* Score columns the planner chose for this batch (see RG_CFG_*): how many, and their bytes in HBM. */
 int rg_batch_columns(rg_engine* e, rg_batch* b, uint32_t* n_columns, uint64_t* bytes);
 
+/* ---------------------------------------------------------------- point ranges ---- */
+/* 1-D PointRangeQuery (search/query/point_range_query.rs) as a filter beside the TermQuery clauses.
+ *
+ * rg_points_upload: every point of one 1-D point field of an uploaded leaf, as (docid, packed value) pairs in any
+ * order — what PointValues::intersect hands a visitor that accepts every cell.  A doc may appear several times
+ * (multi-valued).  field: an engine-wide point-field id; packed: n * bytes_per_dim bytes, the sortable big-endian
+ * encoding of IntPoint / LongPoint / FloatPoint / DoublePoint (util/numeric.rs).  RG_EINVAL: the leaf is not
+ * uploaded, bytes_per_dim is not 4 or 8, a docid lies outside [0, max_doc), or (leaf, field) was uploaded before.
+ * A leaf without an upload for a field has no point values for it: PointRangeWeight::create_scorer returns None. */
+int rg_points_upload(rg_engine* e, uint32_t seg_ord, uint32_t field, uint32_t bytes_per_dim, const int32_t* docs,
+                     const uint8_t* packed, size_t n);
+
+/* One range, bounds inclusive, as PointRangeQuery's pack() writes them (the first bytes_per_dim bytes are used). */
+typedef struct {
+    uint32_t field;
+    uint32_t bytes_per_dim; /* 4 or 8; must equal the field's in every leaf that has it (else RG_EINVAL) */
+    uint8_t lower[8];
+    uint8_t upper[8];
+} rg_point_range;
+
+/* A clause whose occur has this bit set is a range: term_id indexes the rg_point_range array, weight must be +0.0f
+ * (the reference never normalises the weight of a PointRangeWeight, so it scores 0f32; a boosted range is
+ * RG_EUNSUPPORTED) and cache_id is ignored.  Only the *_ranges entry points read it; elsewhere such an occur is an
+ * unknown occur.  Accepted: MUST / FILTER ranges beside MUST / FILTER / SHOULD terms (a conjunction, or the required
+ * side of a ReqOptScorer), MUST_NOT ranges beside required clauses, and a query that is or collapses to one range.
+ * RG_EUNSUPPORTED: SHOULD ranges in a disjunction or beside a MUST, ranges in RG_Q_DISMAX, and MUST_NOT ranges
+ * on a disjunction or beside only MUST_NOT clauses. */
+#define RG_CLAUSE_RANGE 0x100
+
+int rg_batch_prepare_ranges(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                            uint32_t n_clauses, const rg_search_params* p, const rg_point_range* ranges,
+                            uint32_t n_ranges, rg_batch** out);
+int rg_search_batch_ranges(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                           uint32_t n_clauses, const rg_search_params* p, const rg_point_range* ranges,
+                           uint32_t n_ranges, rg_hit* out_hits, uint32_t* out_counts, uint64_t* out_total_hits);
+/* Range-lead blocks of 128 docids in the last run of b: [0] skipped without a read (wholly outside the range),
+ * [1] taken whole without a key read (wholly inside, every doc has a value), [2] scanned key by key. */
+int rg_batch_range_stats(rg_engine* e, rg_batch* b, uint64_t out[3]);
+
 /* ---------------------------------------------------------------- rescoring ------- */
 /* QueryRescorer::rescore (search/scorer/rescorer.rs:130-607) for score TopDocs: the first window_size hits of a
  * row are sorted by docid, scored by a second query (advance() per hit, one scorer per leaf; a hit matches iff the

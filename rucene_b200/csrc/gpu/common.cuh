@@ -65,6 +65,7 @@ struct ItemClause {
                        // bit4: no usable score bound: weight < 0 / NaN or a norm cache with negative entries
                        // bit5: block stream of a term that has a presence bitmap: bits [16, 32) index EvalParams::cols (.bits)
                        // bit3: meta entry after a DisjunctionMaxScorer item's clauses: weight = tie breaker
+                       // bit8: point range — term_id indexes RangeParams::ranges (k_eval_and_ranges only)
 };
 
 struct WorkItem {
@@ -75,6 +76,25 @@ struct WorkItem {
     int32_t lo, hi;          // docid range [lo, hi) inside the segment
     uint32_t clause_begin;   // into ItemClause[]
     uint32_t chain_pos;      // position inside its heap chain (0 = first: no theta to inherit)
+};
+
+// ------------------------------------------------------------------ 1-D point ranges
+// Points of one (leaf, field): keys are the packed sortable bytes read as a big-endian unsigned integer (u32 for 4
+// bytes, u64 for 8), which orders exactly as the byte strings compare.  CSR in docid order: the keys of doc d are
+// keys[offsets[d], offsets[d + 1]), ascending.  One RangeBlock per 128 docids.
+struct RangeBlock {
+    uint64_t min, max;  // smallest / largest key in the block (meaningless when values == 0)
+    uint32_t docs;      // docids of the block with at least one value
+    uint32_t values;    // keys of the block
+};
+// one range clause in one leaf (ItemClause flag bit8: term_id indexes RangeParams::ranges)
+struct RangeRef {
+    const uint32_t* offsets;
+    const void* keys;  // uint32_t (wide == 0) or uint64_t (wide == 1)
+    const RangeBlock* blocks;
+    uint64_t lower, upper;  // inclusive
+    uint32_t wide;
+    uint32_t pad;
 };
 
 struct CandRun {  // header slot of a candidate run in the arena (same size as rg_hit)

@@ -831,8 +831,72 @@ float rg_engine_last_kernel_ms(rg_engine* e, const char* which) {
 uint64_t rg_engine_index_bytes(rg_engine* e) {
     uint64_t b = 0;
     if (e)
-        for (auto& s : e->segs) b += s.device_bytes;
+        for (auto& s : e->segs) {
+            b += s.device_bytes;
+            for (auto& f : s.points) b += f.second.bytes();
+        }
     return b;
+}
+
+int rg_points_upload(rg_engine* e, uint32_t seg_ord, uint32_t field, uint32_t bytes_per_dim, const int32_t* docs,
+                     const uint8_t* packed, size_t n) {
+    RG_TRY
+    if (!e || (n && (!docs || !packed))) throw ArgError("null argument");
+    if (seg_ord >= e->segs.size()) throw ArgError("rg_points_upload: leaf not uploaded");
+    if (bytes_per_dim != 4 && bytes_per_dim != 8) throw ArgError("rg_points_upload: bytes_per_dim must be 4 or 8");
+    Segment& seg = e->segs[seg_ord];
+    if (seg.points.count(field)) throw ArgError("rg_points_upload: field already uploaded for this leaf");
+    const int32_t max_doc = seg.max_doc;
+    if (n > 0xffffffffull) throw ArgError("rg_points_upload: more than 2^32 - 1 points");  // offsets are u32
+    for (size_t i = 0; i < n; i++)
+        if (docs[i] < 0 || docs[i] >= max_doc) throw ArgError("rg_points_upload: docid outside [0, max_doc)");
+    RG_CUDA_CHECK(cudaSetDevice(e->device));
+    // the packed bytes as a big-endian unsigned integer: compares exactly as the byte strings do
+    std::vector<uint64_t> key(n);
+    for (size_t i = 0; i < n; i++) {
+        uint64_t v = 0;
+        for (uint32_t j = 0; j < bytes_per_dim; j++) v = v << 8 | packed[i * bytes_per_dim + j];
+        key[i] = v;
+    }
+    // CSR in docid order, keys ascending within a doc
+    std::vector<uint32_t> offsets((size_t)max_doc + 1, 0);
+    for (size_t i = 0; i < n; i++) offsets[(size_t)docs[i] + 1]++;
+    for (size_t d = 0; d < (size_t)max_doc; d++) offsets[d + 1] += offsets[d];
+    std::vector<uint64_t> csr(n);
+    {
+        std::vector<uint32_t> pos(offsets.begin(), offsets.end() - 1);
+        for (size_t i = 0; i < n; i++) csr[pos[(size_t)docs[i]]++] = key[i];
+    }
+    for (size_t d = 0; d < (size_t)max_doc; d++) std::sort(csr.begin() + offsets[d], csr.begin() + offsets[d + 1]);
+    const size_t n_blk = ((size_t)max_doc + kBlock - 1) / kBlock;
+    std::vector<RangeBlock> blocks(n_blk, RangeBlock{~0ull, 0ull, 0u, 0u});
+    for (size_t d = 0; d < (size_t)max_doc; d++) {
+        RangeBlock& b = blocks[d / kBlock];
+        const uint32_t o0 = offsets[d], o1 = offsets[d + 1];
+        if (o0 == o1) continue;
+        b.docs++;
+        b.values += o1 - o0;
+        b.min = std::min(b.min, csr[o0]);
+        b.max = std::max(b.max, csr[o1 - 1]);
+    }
+    PointField pf;
+    pf.bytes_per_dim = bytes_per_dim;
+    cudaStream_t st = e->stream;
+    upload(pf.offsets, offsets.data(), offsets.size(), st);
+    upload(pf.blocks, blocks.data(), blocks.size(), st);
+    std::vector<uint32_t> k32;
+    if (bytes_per_dim == 4) k32.assign(csr.begin(), csr.end());
+    pf.keys.alloc(n * bytes_per_dim);
+    if (n)
+        RG_CUDA_CHECK(cudaMemcpyAsync(pf.keys.p, bytes_per_dim == 8 ? (const void*)csr.data() : (const void*)k32.data(),
+                                      n * bytes_per_dim, cudaMemcpyHostToDevice, st));
+    RG_CUDA_CHECK(cudaStreamSynchronize(st));  // the host vectors go out of scope
+    std::sort(key.begin(), key.end());
+    pf.sorted = std::move(key);
+    seg.points.emplace(field, std::move(pf));
+    e->generation++;  // batches prepared before this upload are stale
+    return RG_OK;
+    RG_CATCH
 }
 
 int rg_segment_upload(rg_engine* e, uint32_t seg_ord, int32_t doc_base, int32_t max_doc,

@@ -2,6 +2,7 @@
 #pragma once
 #include <cuda_runtime.h>
 
+#include <algorithm>
 #include <cstdint>
 #include <deque>
 #include <map>
@@ -125,6 +126,21 @@ struct TermHost {
     int32_t tail_base = 0;   // last doc of the last full block
 };
 
+// the points of one 1-D point field in one leaf (rg_points_upload), see RangeRef
+struct PointField {
+    uint32_t bytes_per_dim = 0;
+    DevBuf<uint32_t> offsets;  // max_doc + 1
+    DevBuf<uint8_t> keys;      // u32 or u64 per point
+    DevBuf<RangeBlock> blocks; // one per 128 docids
+    std::vector<uint64_t> sorted;  // host: every key, ascending (a range's point count in O(log n) when planning)
+    uint64_t bytes() const { return offsets.bytes() + keys.bytes() + blocks.bytes(); }
+    uint64_t count(uint64_t lower, uint64_t upper) const {
+        if (lower > upper) return 0;
+        return (uint64_t)(std::upper_bound(sorted.begin(), sorted.end(), upper) -
+                          std::lower_bound(sorted.begin(), sorted.end(), lower));
+    }
+};
+
 struct Segment {
     SegDev dev{};
     DevBuf<uint4> arena;
@@ -156,6 +172,7 @@ struct Segment {
     DevBuf<uint32_t> dict_ids;
     uint32_t dict_n = 0;
     bool has_dict = false;
+    std::map<uint32_t, PointField> points;  // point field id -> its points in this leaf
     int32_t doc_base = 0, max_doc = 0;
     uint64_t device_bytes = 0;
 };
@@ -228,6 +245,13 @@ void launch_eval_or_ms(cudaStream_t st, const EvalParams& p, const uint32_t* ite
                        uint32_t max_streams, bool has_live, bool planes);
 void launch_eval_and(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n, bool req_opt,
                      bool has_other_enc);
+// k_eval_and items with a point-range clause (the lead may be a range)
+struct RangeParams {
+    const RangeRef* ranges;
+    unsigned long long* blk_stats;  // [3] range-lead blocks skipped, taken whole, scanned
+};
+void launch_eval_and_ranges(cudaStream_t st, const EvalParams& p, const RangeParams& rp, const uint32_t* item_ids,
+                            uint32_t n, bool req_opt, bool has_other_enc);
 
 // rescore.cu: QueryRescorer over TopDocs rows in HBM.  The rescoring query's scorer per (query, leaf), as
 // BooleanWeight::create_scorer builds it; its clauses are ItemClauses (weight = the clause's scoring weight, flags

@@ -589,12 +589,36 @@ struct AndShared {
 // item always covers the whole leaf and one thread replays the chain per step, in docid order.
 constexpr uint32_t kOptScoreThreshold = 100;
 
-// OTHER: some leaf carries EF / BITSET doc blocks (their decoder is compiled out otherwise)
-template <bool REQOPT, bool OTHER>
-__global__ void __launch_bounds__(kEvalThreads, OTHER ? (REQOPT ? 4 : 5) : 0)  // the decoder call must not cost occupancy
-k_eval_and(EvalParams p, const uint32_t* __restrict__ item_ids) {
+// k_eval_and_ranges: the point-range clauses of the item and, when a range leads, the 128-doc blocks of the step
+struct AndSharedR : AndShared {
+    RangeRef rref[kMaxTerms];
+    uint32_t is_rng[kMaxTerms];
+    int32_t rblk[kEvalWarps];  // lead block of each warp this step (-1: none)
+    uint32_t rcur;             // next lead block to look at
+};
+
+// PointRangeIntersectVisitor::visit_by_packed_value over every value of doc d: lower <= key <= upper for any of
+// them (keys ascending within a doc)
+__device__ __forceinline__ bool range_hit(const RangeRef& r, int d) {
+    const uint32_t o0 = __ldg(r.offsets + d), o1 = __ldg(r.offsets + d + 1);
+    for (uint32_t j = o0; j < o1; j++) {
+        const uint64_t key = r.wide ? __ldg(static_cast<const unsigned long long*>(r.keys) + j)
+                                    : (uint64_t)__ldg(static_cast<const uint32_t*>(r.keys) + j);
+        if (key > r.upper) return false;
+        if (key >= r.lower) return true;
+    }
+    return false;
+}
+
+// OTHER: some leaf carries EF / BITSET doc blocks (their decoder is compiled out otherwise).
+// RANGES: the item has point-range clauses (ItemClause bit8); a range that leads walks the item's docids one 128-doc
+// block per warp.  Without it the body is the plain conjunction / ReqOpt kernel, unchanged.
+template <bool REQOPT, bool OTHER, bool RANGES>
+__device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_t* __restrict__ item_ids,
+                                              const RangeParams& rp) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     AndShared& sh = *reinterpret_cast<AndShared*>(smem_raw);
+    AndSharedR& shr = *reinterpret_cast<AndSharedR*>(smem_raw);  // only touched when RANGES
     const uint32_t item_idx = item_ids[blockIdx.x];
     const WorkItem it = p.items[item_idx];
     const SegDev seg = p.segs[it.seg];
@@ -606,7 +630,12 @@ k_eval_and(EvalParams p, const uint32_t* __restrict__ item_ids) {
     if ((int)threadIdx.x < T) {
         const ItemClause c = p.clauses[it.clause_begin + threadIdx.x];
         const bool is_col = (c.flags & 4u) != 0;  // term_id indexes p.cols then (never the lead clause)
-        const TermDev td = is_col ? TermDev{} : seg.terms[c.term_id];
+        const bool is_rng = RANGES && (c.flags & 256u) != 0;  // term_id indexes rp.ranges
+        if (RANGES) {
+            shr.is_rng[threadIdx.x] = is_rng;
+            if (is_rng) shr.rref[threadIdx.x] = rp.ranges[c.term_id];
+        }
+        const TermDev td = (is_col || is_rng) ? TermDev{} : seg.terms[c.term_id];
         TermCtx& tc = sh.term[threadIdx.x];
         sh.term_id[threadIdx.x] = c.term_id;
         sh.is_not[threadIdx.x] = c.flags & 1u;
@@ -625,6 +654,7 @@ k_eval_and(EvalParams p, const uint32_t* __restrict__ item_ids) {
         tc.w1 = __fmul_rn(c.weight, __fadd_rn(p.k1, 1.0f));
     }
     const uint32_t* theta_prev = (it.chain_pos == 0) ? nullptr : p.item_theta + (item_idx - 1);
+    if (RANGES && threadIdx.x == 0) shr.rcur = (uint32_t)lo / kBlock;
     __syncthreads();
 
     const TermCtx& lead = sh.term[0];
@@ -635,74 +665,136 @@ k_eval_and(EvalParams p, const uint32_t* __restrict__ item_ids) {
     float ro_sum = 0.0f;    // ReqOptScorer::scores_sum / scores_num (thread 0)
     uint32_t ro_num = 0;
     uint32_t touched = 0;   // bytes this thread asked for (block parts are charged to lane 0 of the decoding warp)
+    const bool range_lead = RANGES && shr.is_rng[0] != 0;
+    unsigned long long rstat[3] = {0ull, 0ull, 0ull};  // range-lead blocks skipped / whole / scanned (lane 0s)
 
     for (uint32_t b0 = lead.cur;; b0 += kEvalWarps) {
-        // ---- 1. decode this step's lead blocks (one per warp; pseudo-block lead_nb = vint tail)
-        if (b0 > lead_nb || (b0 == lead_nb && !lead_has_tail)) break;
-        {
-            const int first_prev = b0 == 0 ? -1 : __ldg(lead.blk_last + b0 - 1);
-            if (first_prev >= hi - 1) break;
-        }
         uint32_t inherited = 0;
-        if (threadIdx.x == 0 && theta_prev) inherited = ld_volatile_u32(theta_prev);
-        const uint32_t b = b0 + warp;
-        int4 ld = make_int4(kNoMoreDocs, kNoMoreDocs, kNoMoreDocs, kNoMoreDocs);
-        float4 ls = make_float4(0.f, 0.f, 0.f, 0.f);
-        const float lw1 = lead.w1;
-        if (b < lead_nb) {
-            const int prev_last = b == 0 ? -1 : __ldg(lead.blk_last + b - 1);
-            if (prev_last < hi - 1) {
-                const BlockDesc bd = lead.blk_desc[b];
-                const uint4* part = seg.arena + bd.off16;
-                if (lane == 0) touched += 12u + 16u * (((bd.bits >> 16) & 0xffu) + max(1u, (bd.bits >> 8) & 0xffu));
-                int4 dd;
-                if (!OTHER || (bd.bits >> 24) == 0) {
-                    const int4 dl = unpack4(part, (int)(bd.bits & 0xff), lane, seg.version, seg.sb_mask);
-                    dd = deltas_to_docs(dl, b == 0 ? 0 : prev_last);
-                } else {  // EF / BITSET doc part (this warp's ldoc slice is rewritten below)
-                    decode_other_docs_call(part, bd.bits >> 24, b == 0 ? -1 : prev_last, sh.ldoc + warp * kBlock, lane);
-                    dd = reinterpret_cast<const int4*>(sh.ldoc + warp * kBlock)[lane];
-                    __syncwarp();
-                }
-                const int4 fr = unpack4(part + ((bd.bits >> 16) & 0xff), (int)((bd.bits >> 8) & 0xff), lane,
-                                        seg.version, seg.sb_mask);
-                const int docs[4] = {dd.x, dd.y, dd.z, dd.w};
-                const int fq[4] = {fr.x, fr.y, fr.z, fr.w};
-                int od[4];
-                float os[4];
-#pragma unroll
-                for (int i = 0; i < 4; i++) {
-                    const int d = docs[i];
-                    const bool ok = d >= lo && d < hi;
-                    od[i] = ok ? d : kNoMoreDocs;
-                    float s = 0.f;
-                    if (ok) {
-                        const float nrm = seg.norms ? __ldg(lead.cache + __ldg(seg.norms + d)) : p.k1;
-                        s = bm25_score(lw1, (float)fq[i], nrm);
-                        touched += 1u;
+        if (range_lead) {
+            // ---- 1'. range lead: the next kEvalWarps blocks of the item that can hold a match, one per warp, in
+            // docid order.  Warp 0 reads the block table 32 entries at a time and compacts the blocks that overlap
+            // the range (ballot + prefix count); the others are skipped without a key read.
+            const RangeRef& rr = shr.rref[0];
+            const uint32_t rend = (uint32_t)(hi - 1) / kBlock + 1;
+            if (warp == 0) {
+                uint32_t cur = shr.rcur, found = 0;
+                while (found < (uint32_t)kEvalWarps && cur < rend) {
+                    const uint32_t bi = cur + lane;
+                    bool take = false;
+                    if (bi < rend) {
+                        const RangeBlock bk = rr.blocks[bi];
+                        take = bk.values > 0 && bk.max >= rr.lower && bk.min <= rr.upper;
                     }
-                    os[i] = s;
-                }
-                ld = make_int4(od[0], od[1], od[2], od[3]);
-                ls = make_float4(os[0], os[1], os[2], os[3]);
-            }
-            reinterpret_cast<int4*>(sh.ldoc + warp * kBlock)[lane] = ld;
-            reinterpret_cast<float4*>(sh.lscore + warp * kBlock)[lane] = ls;
-        } else {
-            reinterpret_cast<int4*>(sh.ldoc + warp * kBlock)[lane] = ld;
-            reinterpret_cast<float4*>(sh.lscore + warp * kBlock)[lane] = ls;
-            __syncwarp();
-            if (b == lead_nb && lead_has_tail) {
-                if (lane == 0) {
-                    decode_tail(seg, seg.terms[sh.term_id[0]], sh.slab_docs[warp], sh.slab_freqs[warp]);
+                    const uint32_t m = __ballot_sync(0xffffffffu, take);
+                    const uint32_t need = (uint32_t)kEvalWarps - found;
+                    const uint32_t rank = __popc(m & ((1u << lane) - 1u));
+                    if (take && rank < need) shr.rblk[found + rank] = (int32_t)bi;
+                    const uint32_t last = __ballot_sync(0xffffffffu, take && rank == need - 1u);
+                    const uint32_t consumed = last ? (uint32_t)__ffs(last) : min(32u, rend - cur);
+                    const uint32_t got = min((uint32_t)__popc(m), need);
+                    rstat[0] += consumed - got;
+                    found += got;
+                    cur += consumed;
                 }
                 __syncwarp();
-                for (uint32_t j = lane; j < lead.tail_n; j += 32) {
-                    const int d = sh.slab_docs[warp][j];
-                    if (d >= lo && d < hi) {
-                        const float nrm = seg.norms ? __ldg(lead.cache + __ldg(seg.norms + d)) : p.k1;
-                        sh.ldoc[warp * kBlock + j] = d;
-                        sh.lscore[warp * kBlock + j] = bm25_score(lw1, (float)sh.slab_freqs[warp][j], nrm);
+                if (lane == 0) {
+                    for (uint32_t w = found; w < (uint32_t)kEvalWarps; w++) shr.rblk[w] = -1;
+                    shr.rcur = cur;
+                }
+                if (lane != 0) rstat[0] = 0;
+            }
+            __syncthreads();
+            if (shr.rblk[0] < 0) break;
+            if (threadIdx.x == 0 && theta_prev) inherited = ld_volatile_u32(theta_prev);
+            int od[4] = {kNoMoreDocs, kNoMoreDocs, kNoMoreDocs, kNoMoreDocs};
+            const int32_t blk = shr.rblk[warp];
+            if (blk >= 0) {
+                const RangeBlock bk = rr.blocks[blk];
+                const int base = blk * kBlock;
+                // wholly inside the range and every doc of the block has a value: all docids, no key read
+                const bool whole = bk.min >= rr.lower && bk.max <= rr.upper &&
+                                   (int)bk.docs == min(kBlock, seg.max_doc - base);
+                if (lane == 0) {
+                    rstat[whole ? 1 : 2]++;
+                    touched += 24u;
+                }
+#pragma unroll
+                for (int i = 0; i < 4; i++) {
+                    const int d = base + lane * 4 + i;
+                    if (d >= lo && d < hi && (whole || range_hit(rr, d))) od[i] = d;
+                }
+                if (!whole) touched += 128u;
+            }
+            // ConstantScoreScorer(0): the lead scores +0.0f
+            reinterpret_cast<int4*>(sh.ldoc + warp * kBlock)[lane] = make_int4(od[0], od[1], od[2], od[3]);
+            reinterpret_cast<float4*>(sh.lscore + warp * kBlock)[lane] = make_float4(0.f, 0.f, 0.f, 0.f);
+        } else {
+            // ---- 1. decode this step's lead blocks (one per warp; pseudo-block lead_nb = vint tail)
+            if (b0 > lead_nb || (b0 == lead_nb && !lead_has_tail)) break;
+            {
+                const int first_prev = b0 == 0 ? -1 : __ldg(lead.blk_last + b0 - 1);
+                if (first_prev >= hi - 1) break;
+            }
+            if (threadIdx.x == 0 && theta_prev) inherited = ld_volatile_u32(theta_prev);
+            const uint32_t b = b0 + warp;
+            int4 ld = make_int4(kNoMoreDocs, kNoMoreDocs, kNoMoreDocs, kNoMoreDocs);
+            float4 ls = make_float4(0.f, 0.f, 0.f, 0.f);
+            const float lw1 = lead.w1;
+            if (b < lead_nb) {
+                const int prev_last = b == 0 ? -1 : __ldg(lead.blk_last + b - 1);
+                if (prev_last < hi - 1) {
+                    const BlockDesc bd = lead.blk_desc[b];
+                    const uint4* part = seg.arena + bd.off16;
+                    if (lane == 0) touched += 12u + 16u * (((bd.bits >> 16) & 0xffu) + max(1u, (bd.bits >> 8) & 0xffu));
+                    int4 dd;
+                    if (!OTHER || (bd.bits >> 24) == 0) {
+                        const int4 dl = unpack4(part, (int)(bd.bits & 0xff), lane, seg.version, seg.sb_mask);
+                        dd = deltas_to_docs(dl, b == 0 ? 0 : prev_last);
+                    } else {  // EF / BITSET doc part (this warp's ldoc slice is rewritten below)
+                        decode_other_docs_call(part, bd.bits >> 24, b == 0 ? -1 : prev_last, sh.ldoc + warp * kBlock, lane);
+                        dd = reinterpret_cast<const int4*>(sh.ldoc + warp * kBlock)[lane];
+                        __syncwarp();
+                    }
+                    const int4 fr = unpack4(part + ((bd.bits >> 16) & 0xff), (int)((bd.bits >> 8) & 0xff), lane,
+                                            seg.version, seg.sb_mask);
+                    const int docs[4] = {dd.x, dd.y, dd.z, dd.w};
+                    const int fq[4] = {fr.x, fr.y, fr.z, fr.w};
+                    int od[4];
+                    float os[4];
+#pragma unroll
+                    for (int i = 0; i < 4; i++) {
+                        const int d = docs[i];
+                        const bool ok = d >= lo && d < hi;
+                        od[i] = ok ? d : kNoMoreDocs;
+                        float s = 0.f;
+                        if (ok) {
+                            const float nrm = seg.norms ? __ldg(lead.cache + __ldg(seg.norms + d)) : p.k1;
+                            s = bm25_score(lw1, (float)fq[i], nrm);
+                            touched += 1u;
+                        }
+                        os[i] = s;
+                    }
+                    ld = make_int4(od[0], od[1], od[2], od[3]);
+                    ls = make_float4(os[0], os[1], os[2], os[3]);
+                }
+                reinterpret_cast<int4*>(sh.ldoc + warp * kBlock)[lane] = ld;
+                reinterpret_cast<float4*>(sh.lscore + warp * kBlock)[lane] = ls;
+            } else {
+                reinterpret_cast<int4*>(sh.ldoc + warp * kBlock)[lane] = ld;
+                reinterpret_cast<float4*>(sh.lscore + warp * kBlock)[lane] = ls;
+                __syncwarp();
+                if (b == lead_nb && lead_has_tail) {
+                    if (lane == 0) {
+                        decode_tail(seg, seg.terms[sh.term_id[0]], sh.slab_docs[warp], sh.slab_freqs[warp]);
+                    }
+                    __syncwarp();
+                    for (uint32_t j = lane; j < lead.tail_n; j += 32) {
+                        const int d = sh.slab_docs[warp][j];
+                        if (d >= lo && d < hi) {
+                            const float nrm = seg.norms ? __ldg(lead.cache + __ldg(seg.norms + d)) : p.k1;
+                            sh.ldoc[warp * kBlock + j] = d;
+                            sh.lscore[warp * kBlock + j] = bm25_score(lw1, (float)sh.slab_freqs[warp][j], nrm);
+                        }
                     }
                 }
             }
@@ -719,6 +811,23 @@ k_eval_and(EvalParams p, const uint32_t* __restrict__ item_ids) {
             const float w1 = tc.w1;
             const bool neg = sh.is_not[t] != 0;
             const bool opt = REQOPT && sh.is_opt[t] != 0;
+            if (RANGES && shr.is_rng[t]) {
+                // range probe: a required range keeps the doc and adds its +0.0f (which turns a -0.0f sum into
+                // +0.0f, as in the reference); a MUST_NOT range drops it.  Ranges are never on the optional side.
+                const RangeRef& rr = shr.rref[t];
+#pragma unroll
+                for (int r = 0; r < kAndSteps; r++) {
+                    const int slot = warp * kBlock + r * 32 + lane;
+                    const int d = sh.ldoc[slot];
+                    if (d == kNoMoreDocs) continue;
+                    touched += 8u;
+                    const bool hit = range_hit(rr, d);
+                    if (hit && !neg) sh.lscore[slot] = __fadd_rn(sh.lscore[slot], 0.0f);
+                    else if (hit == neg) sh.ldoc[slot] = kNoMoreDocs;
+                }
+                __syncwarp();
+                continue;
+            }
             if (const float* col = sh.colp[t]) {
                 // the clause's BM25 contributions sit in a docid-indexed column (+0.0f = no posting): no skip
                 // search, no block decode — the same f32 value the stream path would compute
@@ -874,6 +983,21 @@ k_eval_and(EvalParams p, const uint32_t* __restrict__ item_ids) {
     if (threadIdx.x == 0) p.item_matches[item_idx] = sh.emit.matches;
     touched = __reduce_add_sync(0xffffffffu, touched);
     if (lane == 0 && touched) atomicAdd(p.touched, (unsigned long long)touched);
+    if (RANGES && range_lead && lane == 0)
+        for (int i = 0; i < 3; i++)
+            if (rstat[i]) atomicAdd(rp.blk_stats + i, rstat[i]);
+}
+
+template <bool REQOPT, bool OTHER>
+__global__ void __launch_bounds__(kEvalThreads, OTHER ? (REQOPT ? 4 : 5) : 0)  // the decoder call must not cost occupancy
+k_eval_and(EvalParams p, const uint32_t* __restrict__ item_ids) {
+    eval_and_body<REQOPT, OTHER, false>(p, item_ids, RangeParams{});
+}
+
+template <bool REQOPT, bool OTHER>
+__global__ void __launch_bounds__(kEvalThreads, OTHER ? (REQOPT ? 4 : 5) : 0)
+k_eval_and_ranges(EvalParams p, const uint32_t* __restrict__ item_ids, RangeParams rp) {
+    eval_and_body<REQOPT, OTHER, true>(p, item_ids, rp);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1256,6 +1380,21 @@ void launch_eval_and(cudaStream_t st, const EvalParams& p, const uint32_t* item_
     else if (req_opt) launch_eval_and_t<true, false>(st, p, item_ids, n);
     else if (has_other_enc) launch_eval_and_t<false, true>(st, p, item_ids, n);
     else launch_eval_and_t<false, false>(st, p, item_ids, n);
+}
+template <bool REQOPT, bool OTHER>
+static void launch_eval_and_ranges_t(cudaStream_t st, const EvalParams& p, const RangeParams& rp,
+                                     const uint32_t* item_ids, uint32_t n) {
+    cudaFuncSetAttribute(k_eval_and_ranges<REQOPT, OTHER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)sizeof(AndSharedR));
+    k_eval_and_ranges<REQOPT, OTHER><<<n, kEvalThreads, sizeof(AndSharedR), st>>>(p, item_ids, rp);
+}
+void launch_eval_and_ranges(cudaStream_t st, const EvalParams& p, const RangeParams& rp, const uint32_t* item_ids,
+                            uint32_t n, bool req_opt, bool has_other_enc) {
+    if (!n) return;
+    if (req_opt && has_other_enc) launch_eval_and_ranges_t<true, true>(st, p, rp, item_ids, n);
+    else if (req_opt) launch_eval_and_ranges_t<true, false>(st, p, rp, item_ids, n);
+    else if (has_other_enc) launch_eval_and_ranges_t<false, true>(st, p, rp, item_ids, n);
+    else launch_eval_and_ranges_t<false, false>(st, p, rp, item_ids, n);
 }
 void launch_heap_replay(cudaStream_t st, const ReplayParams& p) {
     if (!p.n_groups) return;

@@ -82,6 +82,11 @@ struct rg_batch {
     cudaEvent_t uploaded = nullptr, done = nullptr, ev[4] = {nullptr, nullptr, nullptr, nullptr};
     bool synced = false;  // the host has waited for `done`
     DevBuf<uint8_t> rescore_plan;  // the last rg_batch_rescore's plan (read by its k_rescore)
+    // point ranges: RangeRef per (leaf, range), the items of k_eval_and_ranges, its block counters (zeroed per run)
+    Span<RangeRef> range_refs;
+    Span<uint32_t> and_rng_ids, ro_rng_ids;
+    uint32_t n_and_rng = 0, n_ro_rng = 0;
+    Span<unsigned long long> range_stats;
     ~rg_batch() {
         for (cudaEvent_t x : {uploaded, done, ev[0], ev[1], ev[2], ev[3]})
             if (x) cudaEventDestroy(x);
@@ -113,6 +118,9 @@ struct HostPlan {
     std::vector<ItemClause> clauses;
     std::vector<uint32_t> or_ids, ms_ids, and_ids, ro_ids, dpq_ids, lean_ids;
     uint32_t max_dpq_terms = 0;
+    // point ranges: RangeRef per (leaf, range); conjunction / ReqOpt items with a range clause (k_eval_and_ranges)
+    std::vector<RangeRef> range_refs;
+    std::vector<uint32_t> and_rng_ids, ro_rng_ids;
     // batch-local scored lists: build jobs whose dst is an offset (in floats) into the batch's list region, and the
     // col_refs entries to point there once the slab exists
     std::vector<ColumnJob> local_jobs;
@@ -134,6 +142,7 @@ struct HostPlan {
     void reset() {
         items.clear(); clauses.clear(); or_ids.clear(); ms_ids.clear(); and_ids.clear(); ro_ids.clear(); dpq_ids.clear();
         lean_ids.clear(); lean_rank.clear(); local_jobs.clear(); local_refs.clear();
+        range_refs.clear(); and_rng_ids.clear(); ro_rng_ids.clear();
         local_floats = 0;
         local_units = 0;
         col_refs.clear(); bitmap_refs.clear(); cols.clear(); lists.clear(); or_rank.clear(); ms_rank.clear(); and_rank.clear();
@@ -160,7 +169,76 @@ struct QShape {
     float tie = 0.0f;
     std::vector<uint32_t> opt_idx;     // SHOULD clauses beside a MUST (ReqOptScorer's optional side), clause order
     bool match_all = false;            // only MUST_NOT clauses: BooleanQuery::build adds MatchAllDocsQuery (score 0)
+    // point ranges (RG_CLAUSE_RANGE, only from the *_ranges entry points): required (MUST / FILTER, or the one clause
+    // a query collapses to) and MUST_NOT ones.  A shape with ranges is always kTypeAnd or kTypeReqOpt.
+    std::vector<uint32_t> req_rng, not_rng;
 };
+
+inline bool is_range_clause(const rg_clause& c, const rg_point_range* ranges) {
+    return ranges && (c.occur & RG_CLAUSE_RANGE);
+}
+
+// BooleanQuery::build with PointRangeQuery clauses.  A PointRangeWeight scores 0f32 (its weight is only set by
+// normalize(), which the searcher never calls), so a range is a docid predicate that adds +0.0f: in a conjunction
+// ConjunctionScorer's cost order decides nothing (x + 0.0f == x for every x except -0.0f, which becomes +0.0f
+// wherever the addition happens), and on the required side of a ReqOptScorer made of ranges only the running mean
+// stays 0 and never skips.  Shapes outside that (a range on a disjunction, in a dismax, beside only MUST_NOT
+// clauses) are refused.  Returns false when the query has no range clause (the term-only classify applies).
+bool classify_ranges(const rg_query& q, const rg_clause* clauses, const rg_point_range* ranges, uint32_t n_ranges,
+                     QShape& s) {
+    bool any = false;
+    for (uint32_t i = 0; i < q.n_clauses; i++) {
+        const rg_clause& c = clauses[q.clause_begin + i];
+        if (!is_range_clause(c, ranges)) continue;
+        any = true;
+        if (c.term_id >= n_ranges) throw ArgError("range clause: term_id outside the range array");
+        const rg_point_range& r = ranges[c.term_id];
+        if (r.bytes_per_dim != 4 && r.bytes_per_dim != 8) throw ArgError("range: bytes_per_dim must be 4 or 8");
+        uint32_t wbits;
+        memcpy(&wbits, &c.weight, 4);
+        if (wbits != 0u) throw Unsupported("a boosted PointRangeQuery (weight != +0.0f)");
+    }
+    if (!any) return false;
+    if (q.flags & RG_Q_DISMAX) throw Unsupported("a PointRangeQuery in a DisjunctionMaxQuery");
+    if (!(q.flags & RG_Q_BOOLEAN)) {
+        if (q.n_clauses != 1) throw ArgError("a bare query has exactly one clause");
+        s.type = kTypeAnd;
+        s.req_rng.push_back(q.clause_begin);
+        return true;
+    }
+    if (q.n_clauses > (uint32_t)kMaxTerms) throw Unsupported("more than 9 clauses with a PointRangeQuery");
+    std::vector<uint32_t> musts, shoulds, must_nots, should_rng;
+    for (uint32_t i = 0; i < q.n_clauses; i++) {
+        const uint32_t ci = q.clause_begin + i;
+        const rg_clause& c = clauses[ci];
+        const bool rng = is_range_clause(c, ranges);
+        const int32_t occ = rng ? (c.occur & ~RG_CLAUSE_RANGE) : c.occur;
+        if (occ == RG_MUST || occ == RG_FILTER) (rng ? s.req_rng : musts).push_back(ci);
+        else if (occ == RG_SHOULD) (rng ? should_rng : shoulds).push_back(ci);
+        else if (occ == RG_MUST_NOT) (rng ? s.not_rng : must_nots).push_back(ci);
+        else throw ArgError("unknown occur");
+    }
+    // FILTER terms follow the MUST terms (must_weights, :96-125): keep that order among the terms
+    std::vector<uint32_t> req_terms;
+    for (uint32_t ci : musts)
+        if (clauses[ci].occur == RG_MUST) req_terms.push_back(ci);
+    for (uint32_t ci : musts)
+        if (clauses[ci].occur == RG_FILTER) req_terms.push_back(ci);
+    const size_t n_pos = req_terms.size() + s.req_rng.size() + shoulds.size() + should_rng.size();
+    if (must_nots.empty() && s.not_rng.empty() && n_pos == 1) {  // collapses to the one range (:66-75)
+        s.type = kTypeAnd;
+        if (s.req_rng.empty()) s.req_rng = should_rng;
+        return true;
+    }
+    if (req_terms.empty() && s.req_rng.empty())
+        throw Unsupported("a PointRangeQuery on a disjunction or beside only MUST_NOT clauses");
+    if (!should_rng.empty()) throw Unsupported("a SHOULD PointRangeQuery beside a required clause");
+    s.type = shoulds.empty() ? kTypeAnd : kTypeReqOpt;
+    s.clause_idx = req_terms;
+    s.opt_idx = shoulds;
+    s.not_idx = must_nots;
+    return true;
+}
 
 // what a clause scores with: a FILTER clause is a required clause with NonScoringSimilarity, i.e. exactly 0f32
 // (= BM25 with weight +0: 0 * (k1+1) * f / (f + norm) = +0 for any finite norm)
@@ -272,7 +350,7 @@ bool resolve_leaf(const QShape& shape, const Segment& seg, const rg_clause* clau
         if (df > 0) present.push_back(ci);
         else if (shape.type != kTypeOr) dead = true;  // create_scorer -> None (:201-206)
     }
-    if (dead || (present.empty() && !shape.match_all)) return false;
+    if (dead || (present.empty() && !shape.match_all && shape.req_rng.empty())) return false;
     if (shape.type == kTypeOr && shape.msm > present.size()) return false;  // nothing can reach msm here
     for (uint32_t ci : shape.not_idx) {
         const uint32_t t = clauses[ci].term_id;
@@ -288,6 +366,44 @@ bool resolve_leaf(const QShape& shape, const Segment& seg, const rg_clause* clau
             return seg.host_terms[clauses[a].term_id].doc_freq < seg.host_terms[clauses[b].term_id].doc_freq;
         });
     }
+    return true;
+}
+
+const PointField* point_field(const Segment& seg, const rg_point_range& r) {
+    const auto it = seg.points.find(r.field);
+    if (it == seg.points.end()) return nullptr;
+    if (it->second.bytes_per_dim != r.bytes_per_dim)
+        throw ArgError("range: the field was uploaded with another bytes_per_dim");  // as PointRangeWeight bails
+    return &it->second;
+}
+
+uint64_t be_key(const uint8_t* b, uint32_t n) {
+    uint64_t v = 0;
+    for (uint32_t j = 0; j < n; j++) v = v << 8 | b[j];
+    return v;
+}
+
+// PointRangeWeight::create_scorer per leaf: None when the leaf has no points of the field.  req: the required ranges
+// with their point counts in the leaf (a required range with no points, or none inside it, leaves the leaf without a
+// match: false); nots: the MUST_NOT ranges that can exclude something.
+bool resolve_ranges(const QShape& shape, const Segment& seg, const rg_clause* clauses, const rg_point_range* ranges,
+                    std::vector<std::pair<uint64_t, uint32_t>>& req, std::vector<uint32_t>& nots) {
+    req.clear();
+    nots.clear();
+    for (uint32_t ci : shape.req_rng) {
+        const rg_point_range& r = ranges[clauses[ci].term_id];
+        const PointField* pf = point_field(seg, r);
+        const uint64_t n = pf ? pf->count(be_key(r.lower, r.bytes_per_dim), be_key(r.upper, r.bytes_per_dim)) : 0;
+        if (n == 0) return false;
+        req.emplace_back(n, ci);
+    }
+    for (uint32_t ci : shape.not_rng) {
+        const rg_point_range& r = ranges[clauses[ci].term_id];
+        const PointField* pf = point_field(seg, r);
+        if (pf && pf->count(be_key(r.lower, r.bytes_per_dim), be_key(r.upper, r.bytes_per_dim))) nots.push_back(ci);
+    }
+    std::stable_sort(req.begin(), req.end(),
+                     [](const std::pair<uint64_t, uint32_t>& a, const std::pair<uint64_t, uint32_t>& b) { return a.first < b.first; });
     return true;
 }
 
@@ -846,12 +962,17 @@ void choose_local_lists(rg_engine* e, const std::vector<QShape>& shapes, const r
 }
 
 void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
-                uint32_t n_clauses, uint32_t mode, float k1, HostPlan& hp, PlanTimer& tm, PlanScratch& scratch) {
+                uint32_t n_clauses, uint32_t mode, float k1, HostPlan& hp, PlanTimer& tm, PlanScratch& scratch,
+                const rg_point_range* ranges, uint32_t n_ranges) {
     const uint32_t n_caches = (uint32_t)(e->h_caches.size() / 256);
     const uint32_t n_segs = (uint32_t)e->segs.size();
     std::vector<QShape> shapes(n_queries);
+    bool any_ranges = false;
     for (uint32_t qi = 0; qi < n_queries; qi++) {
-        shapes[qi] = classify(queries[qi], clauses, n_clauses);
+        if (ranges && (uint64_t)queries[qi].clause_begin + queries[qi].n_clauses > n_clauses)
+            throw ArgError("query clause range out of bounds");
+        if (ranges && classify_ranges(queries[qi], clauses, ranges, n_ranges, shapes[qi])) any_ranges = true;
+        else shapes[qi] = classify(queries[qi], clauses, n_clauses);
         for (uint32_t ci : shapes[qi].clause_idx)
             if (clauses[ci].cache_id >= n_caches) throw ArgError("clause refers to an unset norm cache");
         for (uint32_t ci : shapes[qi].opt_idx)
@@ -893,6 +1014,20 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
             or_grid[si] = std::min<uint32_t>(g, (uint32_t)max_ranges);
         }
     }
+    // every (leaf, range) pair: the range clauses of leaf si point at entry si * n_ranges + range
+    if (any_ranges) {
+        hp.range_refs.assign((size_t)n_segs * n_ranges, RangeRef{});
+        for (uint32_t si = 0; si < n_segs; si++)
+            for (uint32_t ri = 0; ri < n_ranges; ri++) {
+                const rg_point_range& r = ranges[ri];
+                const PointField* pfp = point_field(e->segs[si], r);  // a bytes_per_dim mismatch is RG_EINVAL here
+                if (!pfp) continue;
+                const PointField& pf = *pfp;
+                hp.range_refs[(size_t)si * n_ranges + ri] =
+                    RangeRef{pf.offsets.p, pf.keys.p, pf.blocks.p, be_key(r.lower, r.bytes_per_dim),
+                             be_key(r.upper, r.bytes_per_dim), pf.bytes_per_dim == 8 ? 1u : 0u, 0u};
+            }
+    }
     tm.mark("classify");
     const std::map<ColKey, uint32_t> columns = choose_columns(e, shapes, clauses, k1, hp, tm);
     tm.mark("columns");
@@ -919,6 +1054,18 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
             std::vector<uint32_t> present, nots, opts;
             const bool new_group = mode == RG_MODE_SEARCH_PARALLEL || !group_open;
             if (!resolve_leaf(shape, seg, clauses, present, nots, opts)) continue;
+            // point ranges: the required ones with their point counts (cheapest first) and the MUST_NOT ones
+            std::vector<std::pair<uint64_t, uint32_t>> rreq;
+            std::vector<uint32_t> rnots;
+            if ((!shape.req_rng.empty() || !shape.not_rng.empty()) &&
+                !resolve_ranges(shape, seg, clauses, ranges, rreq, rnots))
+                continue;
+            // the cheapest required clause leads: a range's cost is its point count in the leaf, a term's its df
+            const bool range_lead =
+                !rreq.empty() && (present.empty() || rreq[0].first < (uint64_t)seg.host_terms[clauses[present[0]].term_id].doc_freq);
+            auto range_clause = [&](uint32_t ci, uint32_t not_flag) {
+                return ItemClause{si * n_ranges + clauses[ci].term_id, 0.0f, 0u, 256u | not_flag};
+            };
             // no SHOULD scorer in this leaf -> the MUST side alone, no ReqOptScorer (:259-266)
             // ten or more sub-scorers in this leaf: DisjunctionSumScorer / DisjunctionMaxScorer switch to the
             // DisiPriorityQueue (disjunction_scorer.rs:41-45,118-139), whose summation order only k_eval_dpq reproduces
@@ -928,6 +1075,11 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
             uint64_t cost = 0, bytes = 0, total_df = 0;
             if (shape.match_all) {
                 cost = total_df = (uint64_t)seg.max_doc;  // AllDocsIterator: every docid of the leaf
+            } else if (range_lead) {
+                cost = total_df = rreq[0].first;
+                bytes = 24ull * ((uint64_t)(seg.max_doc + kBlock - 1) / kBlock) + 8ull * cost;  // block table + keys
+                for (uint32_t ci : present) bytes += seg.host_terms[clauses[ci].term_id].enc_bytes;
+                for (uint32_t ci : opts) bytes += seg.host_terms[clauses[ci].term_id].enc_bytes;
             } else if (shape.type != kTypeOr) {
                 cost = (uint64_t)seg.host_terms[clauses[present[0]].term_id].doc_freq;
                 const TermHost& lead = seg.host_terms[clauses[present[0]].term_id];
@@ -1027,24 +1179,30 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
             } else {
                 // conjunction: the lead (cheapest) clause is a block stream; every other clause that has a score
                 // column is probed by one gather per lead doc instead of skip search + block decode
+                // a range that leads comes first; the other required ranges are probed after the terms (each adds
+                // +0.0f, so where it is added does not change the sum)
+                if (range_lead) lp.clauses.push_back(range_clause(rreq[0].second, 0u));
                 for (size_t i = 0; i < present.size(); i++) {
                     const rg_clause& c = clauses[present[i]];
-                    const int64_t col = i == 0 ? -1 : col_of(present[i]);
+                    const int64_t col = (i == 0 && !range_lead) ? -1 : col_of(present[i]);
                     if (col >= 0) lp.clauses.push_back(ItemClause{(uint32_t)col, clause_weight(c), c.cache_id, 4u});
                     else lp.clauses.push_back(ItemClause{c.term_id, clause_weight(c), c.cache_id, 0});
                 }
+                for (size_t i = range_lead ? 1 : 0; i < rreq.size(); i++) lp.clauses.push_back(range_clause(rreq[i].second, 0u));
             }
             for (uint32_t ci : nots) {
                 const int64_t col = shape.type == kTypeOr ? -1 : col_of(ci);  // conjunctions: any column of the term will do
                 if (col >= 0) lp.clauses.push_back(ItemClause{(uint32_t)col, 0.0f, clauses[ci].cache_id, 1u | 4u});
                 else lp.clauses.push_back(ItemClause{clauses[ci].term_id, 0.0f, clauses[ci].cache_id, 1u});
             }
+            for (uint32_t ci : rnots) lp.clauses.push_back(range_clause(ci, 1u));
             for (uint32_t ci : opts) {
                 const int64_t col = col_of(ci);
                 if (col >= 0) lp.clauses.push_back(ItemClause{(uint32_t)col, clauses[ci].weight, clauses[ci].cache_id, 2u | 4u});
                 else lp.clauses.push_back(ItemClause{clauses[ci].term_id, clauses[ci].weight, clauses[ci].cache_id, 2u});
             }
-            const uint32_t n_item_terms = (uint32_t)(present.size() + (shape.match_all ? 1 : 0) + nots.size() + opts.size());
+            const uint32_t n_item_terms =
+                (uint32_t)(present.size() + (shape.match_all ? 1 : 0) + nots.size() + opts.size() + rreq.size() + rnots.size());
             // DisjunctionMaxWeight::create_scorer (disjunction_max_query.rs:135-155): one scorer in this
             // leaf is that scorer; otherwise the tie breaker rides in a meta clause after the item's
             const bool leaf_dismax = shape.dismax && present.size() > 1;
@@ -1066,7 +1224,11 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
                 }
             }
             R = std::max<uint64_t>(1, std::min<uint64_t>(R, (uint64_t)(seg.max_doc + kBlock - 1) / kBlock));
-            if (leaf_type == (int)kTypeReqOpt || leaf_dpq) R = 1;  // sequential scorer state: one item per leaf
+            // sequential scorer state: one item per leaf.  Except a ReqOptScorer whose required side is only ranges:
+            // its required score is +0.0f, so scores_sum stays 0, 2 * 0 < 0 never holds and the running mean never
+            // skips the optional side — the docid ranges are independent
+            if ((leaf_type == (int)kTypeReqOpt && !present.empty()) || leaf_dpq) R = 1;
+            const uint64_t n_lead_blocks = (uint64_t)(seg.max_doc + kBlock - 1) / kBlock;
             if (new_group) {
                 // SEARCH: one heap per query over all its leaves; SEARCH_PARALLEL: one per leaf
                 lp.group_out.push_back(mode == RG_MODE_SEARCH_PARALLEL ? si * n_queries + qi : qi);
@@ -1080,6 +1242,10 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
                 it.n_terms = (uint8_t)n_item_terms;
                 it.lo = (int32_t)((uint64_t)seg.max_doc * r / R);
                 it.hi = (int32_t)((uint64_t)seg.max_doc * (r + 1) / R);
+                if (range_lead) {  // a range lead walks whole 128-doc blocks: cut on block edges
+                    it.lo = (int32_t)(n_lead_blocks * r / R * kBlock);
+                    it.hi = r + 1 == R ? seg.max_doc : (int32_t)(n_lead_blocks * (r + 1) / R * kBlock);
+                }
                 it.clause_begin = clause_begin;
                 it.chain_pos = (r == 0 && new_group) ? 0u : chain_pos;
                 chain_pos = it.chain_pos + 1;
@@ -1215,6 +1381,20 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
     by_rank(hp.ms_ids, hp.ms_rank);
     by_rank(hp.lean_ids, hp.lean_rank);
     by_rank(hp.and_ids, hp.and_rank);
+    if (any_ranges) {  // items with a range clause go to k_eval_and_ranges, in the same launch order
+        auto split = [&](std::vector<uint32_t>& ids, std::vector<uint32_t>& rng_ids) {
+            std::vector<uint32_t> keep;
+            for (uint32_t id : ids) {
+                const WorkItem& it = hp.items[id];
+                bool r = false;
+                for (uint32_t c = 0; c < it.n_terms; c++) r = r || (hp.clauses[it.clause_begin + c].flags & 256u) != 0;
+                (r ? rng_ids : keep).push_back(id);
+            }
+            ids.swap(keep);
+        };
+        split(hp.and_ids, hp.and_rng_ids);
+        split(hp.ro_ids, hp.ro_rng_ids);
+    }
     // heap groups = contiguous item runs starting at chain-start items
     for (uint32_t i = 0; i < hp.items.size(); i++)
         if (hp.items[i].chain_pos == 0) hp.group_item_begin.push_back(i);
@@ -1347,9 +1527,9 @@ void ensure_arena(rg_engine* e) {
 
 extern "C" {
 
-int rg_batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries,
-                     const rg_clause* clauses, uint32_t n_clauses, const rg_search_params* p,
-                     rg_batch** out) {
+static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                         uint32_t n_clauses, const rg_search_params* p, const rg_point_range* ranges, uint32_t n_ranges,
+                         rg_batch** out) {
     RG_TRY
     if (!e || !p || !out || (n_queries && !queries) || (n_clauses && !clauses)) throw ArgError("null argument");
     *out = nullptr;
@@ -1366,7 +1546,7 @@ int rg_batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries,
     PlanScratch& scratch = *static_cast<PlanScratch*>(e->plan_scratch.get());
     HostPlan& hp = scratch.hp;
     hp.reset();
-    plan_batch(e, queries, n_queries, clauses, n_clauses, p->mode, p->k1, hp, tm, scratch);
+    plan_batch(e, queries, n_queries, clauses, n_clauses, p->mode, p->k1, hp, tm, scratch, ranges, n_ranges);
     std::unique_ptr<rg_batch> b(new rg_batch());
     b->generation = e->generation;
     b->cols = std::move(hp.cols);
@@ -1389,6 +1569,8 @@ int rg_batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries,
     b->n_or = (uint32_t)hp.or_ids.size();
     b->n_and = (uint32_t)hp.and_ids.size();
     b->n_ro = (uint32_t)hp.ro_ids.size();
+    b->n_and_rng = (uint32_t)hp.and_rng_ids.size();
+    b->n_ro_rng = (uint32_t)hp.ro_rng_ids.size();
     b->n_groups = (uint32_t)hp.group_out.size();
     b->max_or_terms = hp.max_or_terms;
     b->or_has_not = hp.or_has_not;
@@ -1420,6 +1602,9 @@ int rg_batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries,
     carve(b->local_lists, hp.local_floats / 4);
     carve(b->group_item_begin, hp.group_item_begin.size());
     carve(b->group_out, hp.group_out.size());
+    carve(b->range_refs, hp.range_refs.size());
+    carve(b->and_rng_ids, hp.and_rng_ids.size());
+    carve(b->ro_rng_ids, hp.ro_rng_ids.size());
     // running top-k scores of every OR work item (theta inheritance along a heap chain); skipped when it would
     // not fit comfortably (huge batches with k near 1024): theta then falls back to the per-range bound
     b->topk_cap = (std::min<uint32_t>(p->k, 1024u) + 31u) & ~31u;
@@ -1433,6 +1618,7 @@ int rg_batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries,
     carve(b->item_topk_n, b->n_items);
     carve(b->arena_next, 2);
     carve(b->dbg, 16);
+    carve(b->range_stats, 3);
     carve(b->out_hits, (size_t)std::max<uint32_t>(1, n_queries) * p->k);
     carve(b->out_counts, n_queries);
     carve(b->out_total, n_queries);
@@ -1464,6 +1650,7 @@ int rg_batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries,
     rebase(b->group_item_begin); rebase(b->group_out); rebase(b->item_head); rebase(b->item_matches);
     rebase(b->item_theta); rebase(b->item_topk_n); rebase(b->item_topk); rebase(b->arena_next); rebase(b->dbg); rebase(b->out_hits); rebase(b->out_counts);
     rebase(b->out_total);
+    rebase(b->range_refs); rebase(b->and_rng_ids); rebase(b->ro_rng_ids); rebase(b->range_stats);
     if (p->mode == RG_MODE_SEARCH_PARALLEL) rebase(b->leaf_records);
     b->zero_begin = b->slab.p + zero_off;
     b->zero_bytes = off - zero_off;
@@ -1481,6 +1668,9 @@ int rg_batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries,
     up(b->col_refs, hp.col_refs, cs);
     up(b->group_item_begin, hp.group_item_begin, cs);
     up(b->group_out, hp.group_out, cs);
+    up(b->range_refs, hp.range_refs, cs);
+    up(b->and_rng_ids, hp.and_rng_ids, cs);
+    up(b->ro_rng_ids, hp.ro_rng_ids, cs);
     RG_CUDA_CHECK(cudaEventCreateWithFlags(&b->uploaded, cudaEventDisableTiming));
     RG_CUDA_CHECK(cudaEventCreateWithFlags(&b->done, cudaEventDisableTiming));
     for (auto& x : b->ev) RG_CUDA_CHECK(cudaEventCreate(&x));
@@ -1501,15 +1691,35 @@ int rg_batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries,
     }
     b->h2d_bytes = (hp.items.size() * sizeof(WorkItem)) + hp.clauses.size() * sizeof(ItemClause) +
                    4 * (hp.or_ids.size() + hp.lean_ids.size() + hp.ms_ids.size() + hp.dpq_ids.size() + hp.and_ids.size() + hp.ro_ids.size() + hp.group_item_begin.size() + hp.group_out.size()) +
-                   hp.col_refs.size() * sizeof(ColRef);
+                   hp.col_refs.size() * sizeof(ColRef) + hp.range_refs.size() * sizeof(RangeRef) +
+                   4 * (hp.and_rng_ids.size() + hp.ro_rng_ids.size());
     b->kernels_per_run = (b->n_lean ? 1 : 0) + (b->n_ms ? 1 : 0) + (b->n_dpq ? 1 : 0) + (b->n_or ? 1 : 0) + (b->n_and ? 1 : 0) + (b->n_ro ? 1 : 0) + (b->n_groups ? 1 : 0) +
-                         (p->mode == RG_MODE_SEARCH_PARALLEL ? 1 : 0);
+                         (p->mode == RG_MODE_SEARCH_PARALLEL ? 1 : 0) + (b->n_and_rng ? 1 : 0) + (b->n_ro_rng ? 1 : 0);
     tm.mark("alloc_copy_issue");
     RG_CUDA_CHECK(cudaStreamSynchronize(cs));  // the host vectors go out of scope (a running batch is not waited for)
     tm.mark("sync");
     *out = b.release();
     return RG_OK;
     RG_CATCH
+}
+
+int rg_batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries,
+                     const rg_clause* clauses, uint32_t n_clauses, const rg_search_params* p,
+                     rg_batch** out) {
+    return batch_prepare(e, queries, n_queries, clauses, n_clauses, p, nullptr, 0, out);
+}
+
+int rg_batch_prepare_ranges(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                            uint32_t n_clauses, const rg_search_params* p, const rg_point_range* ranges,
+                            uint32_t n_ranges, rg_batch** out) {
+    if (n_ranges && !ranges) {
+        if (out) *out = nullptr;
+        g_last_error = "null argument";
+        return RG_EINVAL;
+    }
+    // a non-null array (even of length 0) makes range clauses readable
+    static const rg_point_range none{};
+    return batch_prepare(e, queries, n_queries, clauses, n_clauses, p, ranges ? ranges : &none, n_ranges, out);
 }
 
 int rg_batch_run(rg_engine* e, rg_batch* b) {
@@ -1561,6 +1771,11 @@ int rg_batch_run(rg_engine* e, rg_batch* b) {
     launch_eval_and(st, ep, b->and_ids.p, b->n_and, false, has_other);
     RG_CUDA_CHECK(cudaGetLastError());
     launch_eval_and(st, ep, b->ro_ids.p, b->n_ro, true, has_other);
+    RG_CUDA_CHECK(cudaGetLastError());
+    const RangeParams rgp{b->range_refs.p, b->range_stats.p};
+    launch_eval_and_ranges(st, ep, rgp, b->and_rng_ids.p, b->n_and_rng, false, has_other);
+    RG_CUDA_CHECK(cudaGetLastError());
+    launch_eval_and_ranges(st, ep, rgp, b->ro_rng_ids.p, b->n_ro_rng, true, has_other);
     RG_CUDA_CHECK(cudaGetLastError());
     RG_CUDA_CHECK(cudaEventRecord(b->ev[3], st));
     ReplayParams rp{};
@@ -1671,6 +1886,38 @@ int rg_search_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries,
                                  out_total_hits + h);
     }
     return rc;
+}
+
+int rg_search_batch_ranges(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                           uint32_t n_clauses, const rg_search_params* p, const rg_point_range* ranges,
+                           uint32_t n_ranges, rg_hit* out_hits, uint32_t* out_counts, uint64_t* out_total_hits) {
+    rg_batch* b = nullptr;
+    int rc = rg_batch_prepare_ranges(e, queries, n_queries, clauses, n_clauses, p, ranges, n_ranges, &b);
+    if (rc != RG_OK) return rc;
+    rc = rg_batch_run(e, b);
+    if (rc == RG_OK) rc = rg_batch_fetch(e, b, out_hits, out_counts, out_total_hits);
+    rg_batch_destroy(e, b);
+    if (rc == RG_ENOMEM && n_queries > 1 && p && p->k) {  // as rg_search_batch
+        const uint32_t h = n_queries / 2;
+        rc = rg_search_batch_ranges(e, queries, h, clauses, n_clauses, p, ranges, n_ranges, out_hits, out_counts,
+                                    out_total_hits);
+        if (rc == RG_OK)
+            rc = rg_search_batch_ranges(e, queries + h, n_queries - h, clauses, n_clauses, p, ranges, n_ranges,
+                                        out_hits + (size_t)h * p->k, out_counts + h, out_total_hits + h);
+    }
+    return rc;
+}
+
+int rg_batch_range_stats(rg_engine* e, rg_batch* b, uint64_t out[3]) {
+    RG_TRY
+    if (!e || !b || !out) throw ArgError("null argument");
+    memset(out, 0, 3 * sizeof(uint64_t));
+    if (b->ran) {
+        RG_CUDA_CHECK(cudaStreamSynchronize(e->stream));
+        RG_CUDA_CHECK(cudaMemcpy(out, b->range_stats.p, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    }
+    return RG_OK;
+    RG_CATCH
 }
 
 int rg_batch_debug(rg_engine* e, rg_batch* b, uint64_t out[16]) {

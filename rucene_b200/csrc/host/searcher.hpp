@@ -9,10 +9,14 @@
 //   search/sort_field/collapse_top_docs.rs:22-68,288-326 ScoreDoc / TopDocs
 //   search/similarity/bm25_similarity.rs:45-46,151-177 BM25Similarity, compute_weight
 //   search/scorer/rescorer.rs:67-115,542-556 RescoreRequest, RescoreMode, QueryRescorer::rescore
+//   search/query/point_range_query.rs  PointRangeQuery, IntPoint / LongPoint / FloatPoint / DoublePoint (1-D; the
+//                                      sortable bytes of util/numeric.rs:163-220)
 // (paths relative to src/core/ of zhihu/rucene).  Header-only; link librucene_gpu.so.
 #pragma once
 #include <algorithm>
 #include <cstdint>
+#include <cstring>
+#include <map>
 #include <memory>
 #include <stdexcept>
 #include <string>
@@ -51,6 +55,58 @@ struct TermQuery : Query {
     float boost;
     TermQuery(Term t, float b) : term(std::move(t)), boost(b) {}
     static QueryPtr create(Term t, float boost = 1.0f) { return std::make_shared<TermQuery>(std::move(t), boost); }
+};
+
+// A 1-D point range, bounds inclusive, as packed sortable bytes (4 or 8).  Scores 0f32: PointRangeWeight's weight is
+// only set by normalize(), which the searcher never calls.
+struct PointRangeQuery : Query {
+    std::string field, lower, upper;
+    PointRangeQuery(std::string f, std::string lo, std::string hi)
+        : field(std::move(f)), lower(std::move(lo)), upper(std::move(hi)) {}
+    static QueryPtr create(std::string field, std::string lower, std::string upper) {
+        if (lower.size() != upper.size() || (lower.size() != 4 && lower.size() != 8))
+            throw IllegalArgument("1-D points of 4 or 8 bytes: lower and upper must have the same length");
+        return std::make_shared<PointRangeQuery>(std::move(field), std::move(lower), std::move(upper));
+    }
+};
+
+namespace detail {
+inline std::string be_bytes(uint64_t v, int n) {
+    std::string out((size_t)n, '\0');
+    for (int i = n - 1; i >= 0; i--, v >>= 8) out[(size_t)i] = (char)(v & 0xff);
+    return out;
+}
+}  // namespace detail
+
+// int_to_sortable_bytes / long_to_sortable_bytes: the sign bit flipped, big-endian
+struct IntPoint {
+    static std::string pack(int32_t v) { return detail::be_bytes((uint32_t)v ^ 0x80000000u, 4); }
+    static QueryPtr new_range_query(std::string f, int32_t lo, int32_t hi) { return PointRangeQuery::create(std::move(f), pack(lo), pack(hi)); }
+    static QueryPtr new_exact_query(std::string f, int32_t v) { return new_range_query(std::move(f), v, v); }
+};
+struct LongPoint {
+    static std::string pack(int64_t v) { return detail::be_bytes((uint64_t)v ^ 0x8000000000000000ull, 8); }
+    static QueryPtr new_range_query(std::string f, int64_t lo, int64_t hi) { return PointRangeQuery::create(std::move(f), pack(lo), pack(hi)); }
+    static QueryPtr new_exact_query(std::string f, int64_t v) { return new_range_query(std::move(f), v, v); }
+};
+// sortable_float_bits / sortable_double_bits: -0.0 < +0.0, NaNs beyond the infinities
+struct FloatPoint {
+    static std::string pack(float f) {
+        int32_t b;
+        std::memcpy(&b, &f, 4);
+        return IntPoint::pack(b ^ ((b >> 31) & 0x7fffffff));
+    }
+    static QueryPtr new_range_query(std::string fl, float lo, float hi) { return PointRangeQuery::create(std::move(fl), pack(lo), pack(hi)); }
+    static QueryPtr new_exact_query(std::string fl, float v) { return new_range_query(std::move(fl), v, v); }
+};
+struct DoublePoint {
+    static std::string pack(double d) {
+        int64_t b;
+        std::memcpy(&b, &d, 8);
+        return LongPoint::pack(b ^ ((b >> 63) & 0x7fffffffffffffffll));
+    }
+    static QueryPtr new_range_query(std::string fl, double lo, double hi) { return PointRangeQuery::create(std::move(fl), pack(lo), pack(hi)); }
+    static QueryPtr new_exact_query(std::string fl, double v) { return new_range_query(std::move(fl), v, v); }
 };
 
 // MatchAllDocsQuery (search/query/match_all_query.rs:28-116): every docid, score 0f32
@@ -173,16 +229,29 @@ public:
     GpuIndexSearcher(const GpuIndexSearcher&) = delete;
     GpuIndexSearcher& operator=(const GpuIndexSearcher&) = delete;
 
+    // The points of one 1-D point field of leaf `leaf` (what PointValues::intersect hands an accept-all visitor):
+    // docs[i] has the packed sortable value packed[i * bytes_per_dim ..].  A field never uploaded has no points.
+    void upload_points(uint32_t leaf, const std::string& field, uint32_t bytes_per_dim, const int32_t* docs,
+                       const uint8_t* packed, size_t n) {
+        auto it = point_fields_.emplace(field, (uint32_t)point_fields_.size()).first;
+        check(rg_points_upload(engine_, leaf, it->second, bytes_per_dim, docs, packed, n));
+    }
+
     // IndexSearcher::search(&query, &mut collector)
     void search(const Query& query, TopDocsCollector& collector) {
         std::vector<rg_clause> clauses;
-        rg_query q = compile(query, clauses);
+        std::vector<rg_point_range> ranges;
+        rg_query q = compile(query, clauses, &ranges);
         const uint32_t k = (uint32_t)collector.estimated_hits();
         std::vector<rg_hit> hits(k);
         uint32_t count = 0;
         uint64_t total = 0;
         rg_search_params p{k, sim_.k1, RG_MODE_SEARCH, 0};
-        check(rg_search_batch(engine_, &q, 1, clauses.data(), (uint32_t)clauses.size(), &p, hits.data(), &count, &total));
+        if (ranges.empty())
+            check(rg_search_batch(engine_, &q, 1, clauses.data(), (uint32_t)clauses.size(), &p, hits.data(), &count, &total));
+        else
+            check(rg_search_batch_ranges(engine_, &q, 1, clauses.data(), (uint32_t)clauses.size(), &p, ranges.data(),
+                                         (uint32_t)ranges.size(), hits.data(), &count, &total));
         std::vector<ScoreDoc> docs(count);
         for (uint32_t i = 0; i < count; i++) docs[i] = ScoreDoc{hits[i].doc, hits[i].score};
         collector.fill(TopDocs(total, std::move(docs)));
@@ -233,18 +302,37 @@ private:
         c.cache_id = 0;
         return c;
     }
-    rg_query compile(const Query& query, std::vector<rg_clause>& clauses) const {
+    // a TermQuery or (ranges != null) a PointRangeQuery as one clause
+    void add_clause(const Query& leaf, int32_t occur, std::vector<rg_clause>& clauses,
+                    std::vector<rg_point_range>* ranges) const {
+        if (auto tq = dynamic_cast<const TermQuery*>(&leaf)) {
+            clauses.push_back(clause_of(*tq, occur));
+            return;
+        }
+        auto pq = dynamic_cast<const PointRangeQuery*>(&leaf);
+        if (!pq) throw UnsupportedQuery("only TermQuery and PointRangeQuery leaves are accelerated");
+        if (!ranges) throw UnsupportedQuery("PointRangeQuery is not accelerated here (rescoring)");
+        rg_point_range r{};
+        auto it = point_fields_.find(pq->field);
+        r.field = it == point_fields_.end() ? 0xffffffffu : it->second;  // no leaf has points of it: no scorer anywhere
+        r.bytes_per_dim = (uint32_t)pq->lower.size();
+        std::memcpy(r.lower, pq->lower.data(), pq->lower.size());
+        std::memcpy(r.upper, pq->upper.data(), pq->upper.size());
+        clauses.push_back(rg_clause{occur | RG_CLAUSE_RANGE, (uint32_t)ranges->size(), 0.0f, 0u});
+        ranges->push_back(r);
+    }
+    rg_query compile(const Query& query, std::vector<rg_clause>& clauses,
+                     std::vector<rg_point_range>* ranges = nullptr) const {
         rg_query q{};
         q.clause_begin = (uint32_t)clauses.size();
-        if (auto tq = dynamic_cast<const TermQuery*>(&query)) {
-            clauses.push_back(clause_of(*tq, RG_SHOULD));
+        if (dynamic_cast<const TermQuery*>(&query) || dynamic_cast<const PointRangeQuery*>(&query)) {
+            add_clause(query, RG_SHOULD, clauses, ranges);
             q.n_clauses = 1;
             return q;
         }
         if (auto cq = dynamic_cast<const ConstantScoreQuery*>(&query)) {  // the lone FILTER clause of build()
-            auto tq = dynamic_cast<const TermQuery*>(cq->query.get());
-            if (!tq || cq->boost != 0.0f) throw UnsupportedQuery("only ConstantScoreQuery(TermQuery, 0) is accelerated");
-            clauses.push_back(clause_of(*tq, RG_FILTER));
+            if (!cq->query || cq->boost != 0.0f) throw UnsupportedQuery("only ConstantScoreQuery(leaf, 0) is accelerated");
+            add_clause(*cq->query, RG_FILTER, clauses, ranges);
             q.n_clauses = 1;
             q.flags = RG_Q_BOOLEAN;
             return q;
@@ -256,11 +344,7 @@ private:
             bq->filter_queries.empty() && !bq->must_not_queries.empty())
             musts.clear();  // the engine reads "only MUST_NOT clauses" as MatchAllDocsQuery minus those terms
         auto add = [&](const std::vector<QueryPtr>& v, int32_t occur) {
-            for (const QueryPtr& c : v) {
-                auto tq = dynamic_cast<const TermQuery*>(c.get());
-                if (!tq) throw UnsupportedQuery("only TermQuery leaves are accelerated");
-                clauses.push_back(clause_of(*tq, occur));
-            }
+            for (const QueryPtr& c : v) add_clause(*c, occur, clauses, ranges);
         };
         add(musts, RG_MUST);
         add(bq->filter_queries, RG_FILTER);
@@ -275,6 +359,7 @@ private:
     std::vector<LeafData> leaves_;
     std::string field_;
     std::unordered_map<std::string, uint32_t> term_ids_;
+    std::map<std::string, uint32_t> point_fields_;  // point field name -> engine-wide id, in upload order
     BM25Similarity sim_;
     rg_engine* engine_ = nullptr;
     int32_t max_doc_ = 0;

@@ -27,6 +27,8 @@ CLAUSE_DTYPE = np.dtype([("occur", "<i4"), ("term_id", "<u4"), ("weight", "<f4")
 QUERY_DTYPE = np.dtype([("clause_begin", "<u4"), ("n_clauses", "<u4"),
                         ("min_should_match", "<i4"), ("flags", "<u4")])
 HIT_DTYPE = np.dtype([("doc", "<i4"), ("score", "<f4")])
+CLAUSE_RANGE = 0x100   # rg_clause.occur bit: a point-range clause, term_id indexes the range array (*_ranges calls)
+RANGE_DTYPE = np.dtype([("field", "<u4"), ("bytes_per_dim", "<u4"), ("lower", "u1", 8), ("upper", "u1", 8)])
 
 
 class Config(C.Structure):
@@ -89,6 +91,12 @@ def lib():
                                   vp, vp]
     L.rg_batch_prepare.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(SearchParams),
                                    C.POINTER(vp)]
+    L.rg_points_upload.argtypes = [vp, C.c_uint32, C.c_uint32, C.c_uint32, vp, vp, C.c_size_t]
+    L.rg_batch_prepare_ranges.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(SearchParams), vp,
+                                          C.c_uint32, C.POINTER(vp)]
+    L.rg_search_batch_ranges.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(SearchParams), vp,
+                                         C.c_uint32, vp, vp, vp]
+    L.rg_batch_range_stats.argtypes = [vp, vp, vp]
     L.rg_batch_run.argtypes = [vp, vp]
     L.rg_batch_fetch.argtypes = [vp, vp, vp, vp, vp]
     L.rg_batch_destroy.argtypes = [vp, vp]
@@ -140,6 +148,12 @@ class Batch:
         _check(lib().rg_batch_fetch(self.engine.h, self.h, _p(hits), _p(counts), _p(total)),
                self.engine.h)
         return hits, counts, total
+
+    def range_stats(self):
+        """Range-lead 128-doc blocks of the last run: skipped, taken whole, scanned."""
+        out = np.zeros(3, np.uint64)
+        _check(lib().rg_batch_range_stats(self.engine.h, self.h, _p(out)), self.engine.h)
+        return {"skipped": int(out[0]), "whole": int(out[1]), "scanned": int(out[2])}
 
     def stats(self):
         out = np.zeros(8, np.uint64)
@@ -332,14 +346,41 @@ class Engine:
                                      _p(counts), _p(total)), self.h)
         return hits, counts, total
 
-    def prepare(self, queries, clauses, k, k1=1.2, mode=MODE_SEARCH):
+    def prepare(self, queries, clauses, k, k1=1.2, mode=MODE_SEARCH, ranges=None):
+        """ranges (RANGE_DTYPE array, may be empty): clauses with CLAUSE_RANGE in occur are point ranges."""
         q = np.ascontiguousarray(queries, dtype=QUERY_DTYPE)
         c = np.ascontiguousarray(clauses, dtype=CLAUSE_DTYPE)
         p = self._params(k, k1, mode)
         h = C.c_void_p()
-        _check(lib().rg_batch_prepare(self.h, _p(q), len(q), _p(c), len(c), C.byref(p), C.byref(h)),
-               self.h)
+        if ranges is None:
+            _check(lib().rg_batch_prepare(self.h, _p(q), len(q), _p(c), len(c), C.byref(p), C.byref(h)),
+                   self.h)
+        else:
+            r = np.ascontiguousarray(ranges, dtype=RANGE_DTYPE)
+            _check(lib().rg_batch_prepare_ranges(self.h, _p(q), len(q), _p(c), len(c), C.byref(p), _p(r), len(r),
+                                                 C.byref(h)), self.h)
         return Batch(self, h.value, len(q), k)
+
+    def search_batch_ranges(self, queries, clauses, ranges, k, k1=1.2, mode=MODE_SEARCH):
+        q = np.ascontiguousarray(queries, dtype=QUERY_DTYPE)
+        c = np.ascontiguousarray(clauses, dtype=CLAUSE_DTYPE)
+        r = np.ascontiguousarray(ranges, dtype=RANGE_DTYPE)
+        hits = np.zeros((len(q), k), HIT_DTYPE)
+        counts = np.zeros(len(q), np.uint32)
+        total = np.zeros(len(q), np.uint64)
+        p = self._params(k, k1, mode)
+        _check(lib().rg_search_batch_ranges(self.h, _p(q), len(q), _p(c), len(c), C.byref(p), _p(r), len(r),
+                                            _p(hits), _p(counts), _p(total)), self.h)
+        return hits, counts, total
+
+    def upload_points(self, seg_ord, field, bytes_per_dim, docs, packed):
+        """Every 1-D point of one field of leaf seg_ord: docs[i] has the packed sortable value packed[i]
+        (uint8 [n, bytes_per_dim]); any order, a doc may repeat."""
+        d = np.ascontiguousarray(docs, dtype=np.int32)
+        v = np.ascontiguousarray(packed, dtype=np.uint8).reshape(-1)
+        if v.size != d.size * bytes_per_dim:
+            raise ValueError("packed must hold len(docs) * bytes_per_dim bytes")
+        _check(lib().rg_points_upload(self.h, seg_ord, field, bytes_per_dim, _p(d), _p(v), d.size), self.h)
 
     # ---- QueryRescorer (rescorer.rs) ----
     @staticmethod

@@ -13,6 +13,8 @@ src/core/ of zhihu/rucene):
     TopDocs / ScoreDoc   search/sort_field/collapse_top_docs.rs:22-68,288-326
     IndexSearcher.search search/searcher.rs:238-240,487-525
     RescoreMode / RescoreRequest / QueryRescorer   search/scorer/rescorer.rs:67-115,130-607
+    PointRangeQuery      search/query/point_range_query.rs (1-D: IntPoint / LongPoint / FloatPoint / DoublePoint
+                         pack, new_range_query, new_exact_query; sortable bytes of util/numeric.rs:163-220)
 
 Everything that touches postings runs on the GPU through the C ABI (engine.py); this module only
 does what Query::create_weight does on the host once per query: collection/term statistics from
@@ -57,6 +59,84 @@ class TermQuery(Query):
 
 class IllegalArgument(ValueError):
     """error::ErrorKind::IllegalArgument"""
+
+
+@dataclass(frozen=True)
+class PointRangeQuery(Query):
+    """A 1-D point range, bounds inclusive, as packed sortable bytes.  It scores 0f32 (PointRangeWeight's weight is
+    only set by normalize(), which the searcher never calls), so on the device it is a docid filter."""
+    field: str
+    lower: bytes
+    upper: bytes
+
+    @property
+    def bytes_per_dim(self):
+        return len(self.lower)
+
+    @staticmethod
+    def new(field, lower_point, upper_point):
+        if len(lower_point) != len(upper_point) or len(lower_point) not in (4, 8):
+            raise IllegalArgument("1-D points of 4 or 8 bytes: lower and upper must have the same length")
+        return PointRangeQuery(field, bytes(lower_point), bytes(upper_point))
+
+
+def _sortable_int_bits(bits):   # NumericUtils::sortable_float_bits on the i32 view of an f32
+    b = np.array([bits], np.uint32).view(np.int32)[0]
+    return int(np.int32(b ^ ((b >> 31) & 0x7FFFFFFF)))
+
+
+def _sortable_long_bits(bits):  # NumericUtils::sortable_double_bits on the i64 view of an f64
+    b = np.array([bits], np.uint64).view(np.int64)[0]
+    return int(np.int64(b ^ ((b >> 63) & 0x7FFFFFFFFFFFFFFF)))
+
+
+class IntPoint:
+    BYTES = 4
+
+    @staticmethod
+    def pack(value):
+        """int_to_sortable_bytes: the sign bit flipped, big-endian"""
+        return ((int(value) & 0xFFFFFFFF) ^ 0x80000000).to_bytes(4, "big")
+
+    @classmethod
+    def new_range_query(cls, field, lower, upper):
+        return PointRangeQuery.new(field, cls.pack(lower), cls.pack(upper))
+
+    @classmethod
+    def new_exact_query(cls, field, value):
+        return cls.new_range_query(field, value, value)
+
+
+class LongPoint(IntPoint):
+    BYTES = 8
+
+    @staticmethod
+    def pack(value):
+        return ((int(value) & 0xFFFFFFFFFFFFFFFF) ^ 0x8000000000000000).to_bytes(8, "big")
+
+
+class FloatPoint(IntPoint):
+    @staticmethod
+    def pack(value):
+        """IntPoint::pack(sortable_float_bits(f.to_bits())): -0.0 < +0.0, NaNs beyond the infinities"""
+        return IntPoint.pack(_sortable_int_bits(int(np.array([value], np.float32).view(np.uint32)[0])))
+
+    @staticmethod
+    def pack_bits(bits):
+        """pack of the f32 with these raw bits (any NaN payload)"""
+        return IntPoint.pack(_sortable_int_bits(int(bits) & 0xFFFFFFFF))
+
+
+class DoublePoint(IntPoint):
+    BYTES = 8
+
+    @staticmethod
+    def pack(value):
+        return LongPoint.pack(_sortable_long_bits(int(np.array([value], np.float64).view(np.uint64)[0])))
+
+    @staticmethod
+    def pack_bits(bits):
+        return LongPoint.pack(_sortable_long_bits(int(bits) & 0xFFFFFFFFFFFFFFFF))
 
 
 @dataclass
@@ -213,6 +293,9 @@ class IndexReader:
     segments: Sequence[codec.Segment]
     term_ids: dict = field(default_factory=dict)   # (field, bytes) -> engine-wide term id
     field_name: str = "body"
+    # 1-D point fields: name -> one entry per leaf, (docs int32 [n], packed uint8 [n, bytes_per_dim]) or None when the
+    # leaf has no points of the field (what PointValues::intersect with an accept-all visitor yields)
+    points: dict = field(default_factory=dict)
 
     def max_doc(self):
         return sum(s.max_doc for s in self.segments)
@@ -246,6 +329,16 @@ class GpuIndexSearcher:
         if not eng:
             for seg in reader.segments:
                 self.engine.upload_segment(seg)
+        # engine-wide point field ids: the fields in name order
+        self._point_fields = {name: i for i, name in enumerate(sorted(reader.points))}
+        if not eng:
+            for name, fid in self._point_fields.items():
+                for ord_, leaf in enumerate(reader.points[name]):
+                    if leaf is not None:
+                        docs, packed = leaf
+                        packed = np.asarray(packed, np.uint8)
+                        self.engine.upload_points(ord_, fid, packed.shape[1], docs, packed)
+        self._ranges = None
         # with_similarity (searcher.rs:306-363): statistics of the largest-max_doc leaf
         # (stable sort descending -> first among equals), max_doc of the whole reader
         segs = list(reader.segments)
@@ -278,6 +371,18 @@ class GpuIndexSearcher:
         begin = len(clauses)
 
         def add(q, occur):
+            if isinstance(q, PointRangeQuery):
+                if self._ranges is None:
+                    raise engine.Unsupported(engine.RG_EUNSUPPORTED, "PointRangeQuery is not accelerated here")
+                # a field no leaf has points of gets an id no leaf was uploaded with: no scorer anywhere
+                fid = self._point_fields.get(q.field, 0xFFFFFFFF)
+                r = np.zeros(1, engine.RANGE_DTYPE)[0]
+                r["field"], r["bytes_per_dim"] = fid, q.bytes_per_dim
+                r["lower"][:q.bytes_per_dim] = np.frombuffer(q.lower, np.uint8)
+                r["upper"][:q.bytes_per_dim] = np.frombuffer(q.upper, np.uint8)
+                clauses.append((occur | engine.CLAUSE_RANGE, len(self._ranges), 0.0, 0))
+                self._ranges.append(r)
+                return
             if not isinstance(q, TermQuery):
                 raise engine.Unsupported(engine.RG_EUNSUPPORTED, "only TermQuery leaves are accelerated")
             if self._resolved is not None:   # ids and doc_freq came from the device dictionary
@@ -291,7 +396,7 @@ class GpuIndexSearcher:
             clauses.append((occur, 0xFFFFFFFF if absent else tid,
                             self.term_weight(None if absent else tid, q.boost), 0))
 
-        if isinstance(query, TermQuery):
+        if isinstance(query, (TermQuery, PointRangeQuery)):
             add(query, engine.SHOULD)
             return (begin, 1, 0, 0)
         if isinstance(query, ConstantScoreQuery):
@@ -354,15 +459,44 @@ class GpuIndexSearcher:
         return (np.array(qs, dtype=engine.QUERY_DTYPE).reshape(-1),
                 np.array(clauses, dtype=engine.CLAUSE_DTYPE).reshape(-1))
 
+    def compile_batch_ranges(self, queries):
+        """compile_batch for queries that may hold PointRangeQuerys: (queries, clauses, ranges) for the *_ranges calls"""
+        self._ranges = []
+        try:
+            q, c = self.compile_batch(queries)
+            return q, c, np.array(self._ranges, dtype=engine.RANGE_DTYPE).reshape(-1)
+        finally:
+            self._ranges = None
+
+    @staticmethod
+    def _has_ranges(queries):
+        def walk(q):
+            if isinstance(q, PointRangeQuery):
+                return True
+            if isinstance(q, ConstantScoreQuery):
+                return walk(q.query)
+            if isinstance(q, BooleanQuery):
+                return any(walk(s) for s in q.must_queries + q.should_queries + q.filter_queries + q.must_not_queries)
+            if isinstance(q, DisjunctionMaxQuery):
+                return any(walk(s) for s in q.disjuncts)
+            return False
+        return any(walk(q) for q in queries)
+
     def search_batch(self, queries, k, mode=engine.MODE_SEARCH, rescore=None):
         """rescore: (rescoring queries, RescoreRequest) — one rescoring query per query, the request's weights,
         mode and window for all: QueryRescorer::rescore on every row on the device before the rows are fetched."""
-        q, c = self.compile_batch(queries)
+        ranges = None
+        if self._has_ranges(queries):
+            q, c, ranges = self.compile_batch_ranges(queries)
+        else:
+            q, c = self.compile_batch(queries)
         if rescore is None:
+            if ranges is not None:
+                return self.engine.search_batch_ranges(q, c, ranges, k, k1=self.similarity.k1, mode=mode)
             return self.engine.search_batch(q, c, k, k1=self.similarity.k1, mode=mode)
         rescore_queries, req = rescore
-        rq, rc = self.compile_batch(rescore_queries)
-        batch = self.engine.prepare(q, c, k, k1=self.similarity.k1, mode=mode)
+        rq, rc = self.compile_batch(rescore_queries)   # rescoring takes no ranges: a PointRangeQuery is refused
+        batch = self.engine.prepare(q, c, k, k1=self.similarity.k1, mode=mode, ranges=ranges)
         try:
             batch.run()
             self.engine.rescore_batch(batch, rq, rc, req.window_size, req.query_weight, req.rescore_weight,
