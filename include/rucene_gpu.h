@@ -265,6 +265,35 @@ int rg_search_batch_ranges(rg_engine* e, const rg_query* queries, uint32_t n_que
  * [1] taken whole without a key read (wholly inside, every doc has a value), [2] scanned key by key. */
 int rg_batch_range_stats(rg_engine* e, rg_batch* b, uint64_t out[3]);
 
+/* ---------------------------------------------------------------- nested groups ---- */
+/* One level of nesting: a clause whose occur has this bit set is a GROUP, a pure-SHOULD BooleanQuery of TermQuerys
+ * (what QueryStringQueryBuilder makes of `+(car | auto) +(repair | fix)`).  term_id indexes the `groups` array of the
+ * *_nested calls; that rg_query has RG_Q_BOOLEAN, its own clause_begin / n_clauses in the same clause array and its
+ * min_should_match (<= 1).  Its members are plain RG_SHOULD term clauses with their own weight (idf * boost) and
+ * cache_id; under a FILTER group the weights are ignored (the group scores 0).  A group's score is 0.0f plus its
+ * members' scores in member order over the members on the doc (DisjunctionSumScorer); a MUST / FILTER group whose
+ * members are all absent from a leaf leaves the leaf without a match, a SHOULD or MUST_NOT one is left out.
+ * Accepted: MUST / FILTER / SHOULD / MUST_NOT groups beside terms and ranges where the query is a conjunction or
+ * a ReqOptScorer (at least one MUST / FILTER clause), and the shapes BooleanQuery::build collapses to a group or a term.
+ * At most 9 clauses per (query, leaf) after MUST_NOT groups are flattened, counting every group member.
+ * RG_EUNSUPPORTED: a group beside only SHOULD clauses (`(a | b) (c | d)`), groups in RG_Q_DISMAX, a MUST, FILTER,
+ * MUST_NOT, range or group member, a group with min_should_match > 1, more than 9 clauses.
+ * RG_EINVAL: a group index outside the array, a member with an unknown occur, a member range out of bounds or
+ * overlapping the query's own clauses or another group of the query.  The other entry points treat the bit as an
+ * unknown occur. */
+#define RG_CLAUSE_GROUP 0x200
+
+int rg_batch_prepare_nested(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                            uint32_t n_clauses, const rg_search_params* p, const rg_point_range* ranges,
+                            uint32_t n_ranges, const rg_query* groups, uint32_t n_groups, rg_batch** out);
+int rg_search_batch_nested(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                           uint32_t n_clauses, const rg_search_params* p, const rg_point_range* ranges,
+                           uint32_t n_ranges, const rg_query* groups, uint32_t n_groups, rg_hit* out_hits,
+                           uint32_t* out_counts, uint64_t* out_total_hits);
+/* Group leads in the last run of b: [0] (query, leaf, docid range) items a group led, [1] member postings merged,
+ * [2] of those, postings on a doc that an earlier member of the group also has (they become holes). */
+int rg_batch_group_stats(rg_engine* e, rg_batch* b, uint64_t out[3]);
+
 /* ---------------------------------------------------------------- rescoring ------- */
 /* QueryRescorer::rescore (search/scorer/rescorer.rs:130-607) for score TopDocs: the first window_size hits of a
  * row are sorted by docid, scored by a second query (advance() per hit, one scorer per leaf; a hit matches iff the

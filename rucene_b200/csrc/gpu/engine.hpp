@@ -252,6 +252,10 @@ struct RangeParams {
 };
 void launch_eval_and_ranges(cudaStream_t st, const EvalParams& p, const RangeParams& rp, const uint32_t* item_ids,
                             uint32_t n, bool req_opt, bool has_other_enc);
+// k_eval_and items with a pure-SHOULD group of terms (they may also have ranges).  gstats: [3] items a group led,
+// postings the group leads merged, postings that fell on a doc an earlier member of the group already had
+void launch_eval_and_nested(cudaStream_t st, const EvalParams& p, const RangeParams& rp, unsigned long long* gstats,
+                            const uint32_t* item_ids, uint32_t n, bool req_opt, bool has_other_enc);
 
 // rescore.cu: QueryRescorer over TopDocs rows in HBM.  The rescoring query's scorer per (query, leaf), as
 // BooleanWeight::create_scorer builds it; its clauses are ItemClauses (weight = the clause's scoring weight, flags

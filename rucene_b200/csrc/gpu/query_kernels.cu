@@ -597,6 +597,22 @@ struct AndSharedR : AndShared {
     uint32_t rcur;             // next lead block to look at
 };
 
+// k_eval_and_nested: pure-SHOULD groups of terms (ItemClause bits 9-11).  A group that leads keeps each member's
+// current decoded block here (one member per warp; apart from slab_docs, which the probes overwrite every step); a
+// group probed after the lead sums its members per slot in gsum.
+struct AndSharedN : AndSharedR {
+    int32_t gdoc[kEvalWarps][kBlock];   // group lead: member m's current block (docids)
+    float gscore[kEvalWarps][kBlock];   // ... and its BM25 scores (a vint tail's freqs until they are scored)
+    float gsum[kAndSlots];              // group probe: DisjunctionSumScorer sum of the slot so far (kSent: none)
+    int32_t gpos[kEvalWarps];           // first entry of the slab not yet merged
+    int32_t gend[kEvalWarps];           // end of this step's entries (docids < gy)
+    int32_t gn[kEvalWarps];             // entries in the slab
+    uint32_t gblk[kEvalWarps];          // next block to decode (nb = the vint tail / singleton)
+    uint32_t gdone[kEvalWarps];         // no block left in [lo, hi)
+    uint32_t grp[kMaxTerms];            // ItemClause bits 9-11 of each clause
+    int32_t gx;                         // this step merges docids from gx on
+};
+
 // PointRangeIntersectVisitor::visit_by_packed_value over every value of doc d: lower <= key <= upper for any of
 // them (keys ascending within a doc)
 __device__ __forceinline__ bool range_hit(const RangeRef& r, int d) {
@@ -613,12 +629,15 @@ __device__ __forceinline__ bool range_hit(const RangeRef& r, int d) {
 // OTHER: some leaf carries EF / BITSET doc blocks (their decoder is compiled out otherwise).
 // RANGES: the item has point-range clauses (ItemClause bit8); a range that leads walks the item's docids one 128-doc
 // block per warp.  Without it the body is the plain conjunction / ReqOpt kernel, unchanged.
-template <bool REQOPT, bool OTHER, bool RANGES>
+// GROUPS: the item has pure-SHOULD groups of terms (ItemClause bits 9-11, see AndSharedN); a group that leads merges
+// its members' postings in docid order.  gstats: group-lead counters (GROUPS only).
+template <bool REQOPT, bool OTHER, bool RANGES, bool GROUPS = false>
 __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_t* __restrict__ item_ids,
-                                              const RangeParams& rp) {
+                                              const RangeParams& rp, unsigned long long* gstats = nullptr) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     AndShared& sh = *reinterpret_cast<AndShared*>(smem_raw);
     AndSharedR& shr = *reinterpret_cast<AndSharedR*>(smem_raw);  // only touched when RANGES
+    AndSharedN& shn = *reinterpret_cast<AndSharedN*>(smem_raw);  // only touched when GROUPS
     const uint32_t item_idx = item_ids[blockIdx.x];
     const WorkItem it = p.items[item_idx];
     const SegDev seg = p.segs[it.seg];
@@ -635,6 +654,7 @@ __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_
             shr.is_rng[threadIdx.x] = is_rng;
             if (is_rng) shr.rref[threadIdx.x] = rp.ranges[c.term_id];
         }
+        if (GROUPS) shn.grp[threadIdx.x] = c.flags & (512u | 1024u | 2048u);
         const TermDev td = (is_col || is_rng) ? TermDev{} : seg.terms[c.term_id];
         TermCtx& tc = sh.term[threadIdx.x];
         sh.term_id[threadIdx.x] = c.term_id;
@@ -667,10 +687,165 @@ __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_
     uint32_t touched = 0;   // bytes this thread asked for (block parts are charged to lane 0 of the decoding warp)
     const bool range_lead = RANGES && shr.is_rng[0] != 0;
     unsigned long long rstat[3] = {0ull, 0ull, 0ull};  // range-lead blocks skipped / whole / scanned (lane 0s)
+    // a group leads when its first member is clause 0; its members are clauses [0, G)
+    int G = 1;
+    const bool group_lead = GROUPS && (shn.grp[0] & 512u) != 0;
+    if (GROUPS && group_lead) {
+        G = 0;
+        while (!(shn.grp[G] & 2048u)) G++;
+        G++;
+        if (warp < G && lane == 0) {
+            shn.gblk[warp] = sh.term[warp].cur;
+            shn.gn[warp] = 0;
+            shn.gpos[warp] = 0;
+            shn.gdone[warp] = 0;
+        }
+        if (threadIdx.x == 0) shn.gx = lo;
+    }
+    unsigned long long gstat[2] = {0ull, 0ull};  // group lead: entries merged, entries that became holes
 
     for (uint32_t b0 = lead.cur;; b0 += kEvalWarps) {
         uint32_t inherited = 0;
-        if (range_lead) {
+        if (GROUPS && group_lead) {
+            // ---- 1''. group lead (DisjunctionSumScorer over the members present in the leaf).  Each member's warp
+            // keeps its current block; a step merges the docids [gx, gy) with gy = one past the smallest last docid
+            // of the live members' blocks, so every member contributes at most one block (<= G * 128 <= kAndSlots
+            // entries) and at least one member uses its block up.  Entries go to their rank in (doc, member) order;
+            // the first entry of a doc carries 0.0f + the members' scores in member order, the others become holes.
+            if (warp < G) {
+                TermCtx& tc = sh.term[warp];
+                int32_t* gd = shn.gdoc[warp];
+                float* gs = shn.gscore[warp];
+                const float w1 = tc.w1;
+                while (shn.gpos[warp] >= shn.gn[warp] && !shn.gdone[warp]) {
+                    const uint32_t b = shn.gblk[warp];
+                    const uint32_t nb = tc.nb;
+                    const int prev_last = b == 0 ? -1 : __ldg(tc.blk_last + b - 1);
+                    int n_in = 0;
+                    if (b < nb && prev_last < hi - 1) {
+                        const BlockDesc bd = tc.blk_desc[b];
+                        const uint4* part = seg.arena + bd.off16;
+                        if (lane == 0) touched += 12u + 16u * (((bd.bits >> 16) & 0xffu) + max(1u, (bd.bits >> 8) & 0xffu));
+                        int4 dd;
+                        if (!OTHER || (bd.bits >> 24) == 0) {
+                            const int4 dl = unpack4(part, (int)(bd.bits & 0xff), lane, seg.version, seg.sb_mask);
+                            dd = deltas_to_docs(dl, b == 0 ? 0 : prev_last);
+                        } else {
+                            decode_other_docs_call(part, bd.bits >> 24, b == 0 ? -1 : prev_last, gd, lane);
+                            dd = reinterpret_cast<const int4*>(gd)[lane];
+                            __syncwarp();
+                        }
+                        const int4 fr = unpack4(part + ((bd.bits >> 16) & 0xff), (int)((bd.bits >> 8) & 0xff), lane,
+                                                seg.version, seg.sb_mask);
+                        const int docs[4] = {dd.x, dd.y, dd.z, dd.w};
+                        const int fq[4] = {fr.x, fr.y, fr.z, fr.w};
+                        float os[4];
+#pragma unroll
+                        for (int i = 0; i < 4; i++) {
+                            const int d = docs[i];
+                            const float nrm = seg.norms ? __ldg(tc.cache + __ldg(seg.norms + d)) : p.k1;
+                            os[i] = bm25_score(w1, (float)fq[i], nrm);
+                        }
+                        reinterpret_cast<int4*>(gd)[lane] = dd;
+                        reinterpret_cast<float4*>(gs)[lane] = make_float4(os[0], os[1], os[2], os[3]);
+                        n_in = kBlock;
+                    } else if (b == nb && tc.tail_n > 0 && (nb == 0 || hi - 1 > tc.tail_base)) {
+                        if (lane == 0) decode_tail(seg, seg.terms[sh.term_id[warp]], gd, reinterpret_cast<int32_t*>(gs));
+                        __syncwarp();
+                        for (uint32_t j = lane; j < tc.tail_n; j += 32) {
+                            const int d = gd[j];
+                            const float nrm = seg.norms ? __ldg(tc.cache + __ldg(seg.norms + d)) : p.k1;
+                            gs[j] = bm25_score(w1, (float)reinterpret_cast<const int32_t*>(gs)[j], nrm);
+                        }
+                        n_in = (int)tc.tail_n;
+                    }
+                    __syncwarp();
+                    if (lane == 0) {
+                        if (n_in == 0) {
+                            shn.gdone[warp] = 1;
+                            shn.gn[warp] = 0;
+                            shn.gpos[warp] = 0;
+                        } else {
+                            int l = 0, h = n_in;  // entries below gx were merged by earlier steps or lie before lo
+                            const int x = shn.gx;
+                            while (l < h) {
+                                const int m = (l + h) >> 1;
+                                if (gd[m] < x) l = m + 1;
+                                else h = m;
+                            }
+                            shn.gn[warp] = n_in;
+                            shn.gpos[warp] = l;
+                            shn.gblk[warp] = b + 1;
+                            touched += (uint32_t)n_in;
+                        }
+                    }
+                    __syncwarp();
+                }
+            }
+            __syncthreads();
+            int y = hi;
+            bool any = false;
+            for (int m = 0; m < G; m++)
+                if (!shn.gdone[m]) {
+                    any = true;
+                    y = min(y, shn.gdoc[m][shn.gn[m] - 1] + 1);
+                }
+            if (!any || shn.gx >= hi) break;
+            if (threadIdx.x == 0 && theta_prev) inherited = ld_volatile_u32(theta_prev);
+            if (warp < G && lane == 0) {
+                int l = shn.gpos[warp], h = shn.gn[warp];
+                while (l < h) {
+                    const int m = (l + h) >> 1;
+                    if (shn.gdoc[warp][m] < y) l = m + 1;
+                    else h = m;
+                }
+                shn.gend[warp] = l;
+            }
+            __syncthreads();
+            int n_all = 0;
+            for (int m = 0; m < G; m++) n_all += shn.gend[m] - shn.gpos[m];
+            if (warp < G) {
+                const int pos = shn.gpos[warp], end = shn.gend[warp];
+                for (int j = pos + lane; j < end; j += 32) {
+                    const int d = shn.gdoc[warp][j];
+                    int rank = j - pos;
+                    bool head = true;
+                    float sum = 0.0f;
+                    for (int m = 0; m < G; m++) {
+                        if (m == warp) {
+                            sum = __fadd_rn(sum, shn.gscore[warp][j]);
+                            continue;
+                        }
+                        const int p0 = shn.gpos[m], e0 = shn.gend[m];
+                        int l = p0, h = e0;
+                        while (l < h) {
+                            const int mid = (l + h) >> 1;
+                            if (shn.gdoc[m][mid] < d) l = mid + 1;
+                            else h = mid;
+                        }
+                        const bool eq = l < e0 && shn.gdoc[m][l] == d;
+                        rank += l - p0;
+                        if (m < warp) {
+                            rank += eq ? 1 : 0;
+                            head = head && !eq;
+                        } else if (eq) {
+                            sum = __fadd_rn(sum, shn.gscore[m][l]);
+                        }
+                    }
+                    sh.ldoc[rank] = head ? d : kNoMoreDocs;
+                    sh.lscore[rank] = head ? sum : 0.0f;
+                    if (!head) gstat[1]++;
+                }
+                if (lane == 0) gstat[0] += (unsigned long long)max(0, end - pos);
+            }
+            for (int s = n_all + (int)threadIdx.x; s < kAndSlots; s += kEvalThreads) {
+                sh.ldoc[s] = kNoMoreDocs;
+                sh.lscore[s] = 0.0f;
+            }
+            __syncthreads();
+            if (warp < G && lane == 0) shn.gpos[warp] = shn.gend[warp];
+            if (threadIdx.x == 0) shn.gx = y;
+        } else if (range_lead) {
             // ---- 1'. range lead: the next kEvalWarps blocks of the item that can hold a match, one per warp, in
             // docid order.  Warp 0 reads the block table 32 entries at a time and compacts the blocks that overlap
             // the range (ballot + prefix count); the others are skipped without a key read.
@@ -803,14 +978,21 @@ __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_
 #pragma unroll
             for (int r = 0; r < kAndSteps; r++) sh.oscore[warp * kBlock + r * 32 + lane] = __uint_as_float(kSent);
         }
+        if (GROUPS) {
+#pragma unroll
+            for (int r = 0; r < kAndSteps; r++) shn.gsum[warp * kBlock + r * 32 + lane] = __uint_as_float(kSent);
+        }
         __syncwarp();
         // ---- 2. every other clause, in cost order; each warp works on its own 128 lead slots
-        for (int t = 1; t < T; t++) {
+        for (int t = GROUPS ? G : 1; t < T; t++) {
             const TermCtx& tc = sh.term[t];
             const uint32_t nb = tc.nb;
             const float w1 = tc.w1;
             const bool neg = sh.is_not[t] != 0;
             const bool opt = REQOPT && sh.is_opt[t] != 0;
+            // a group member: a hit adds into the slot's group sum, a miss keeps the slot (the group decides after
+            // its last member); the MUST_NOT side never has groups (excluding (a | b) is excluding a and b)
+            const bool grp = GROUPS && shn.grp[t] != 0;
             if (RANGES && shr.is_rng[t]) {
                 // range probe: a required range keeps the doc and adds its +0.0f (which turns a -0.0f sum into
                 // +0.0f, as in the reference); a MUST_NOT range drops it.  Ranges are never on the optional side.
@@ -844,10 +1026,13 @@ __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_
                         } else if (opt) {
                             const float o = sh.oscore[slot];
                             sh.oscore[slot] = __fadd_rn(__float_as_uint(o) == kSent ? 0.0f : o, v);
+                        } else if (grp) {
+                            const float o = shn.gsum[slot];
+                            shn.gsum[slot] = __fadd_rn(__float_as_uint(o) == kSent ? 0.0f : o, v);
                         } else {
                             sh.lscore[slot] = __fadd_rn(sh.lscore[slot], v);
                         }
-                    } else if (!neg && !opt) {
+                    } else if (!neg && !opt && !grp) {
                         sh.ldoc[slot] = kNoMoreDocs;
                     }
                 }
@@ -864,7 +1049,7 @@ __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_
                     bi = lower_bound_gallop(tc.blk_last, min(sh.hint[warp][t], nb), nb, d);
                     if (bi == nb && !(tc.tail_n > 0 && (nb == 0 || d > tc.tail_base))) {
                         pending = false;  // beyond the last posting of this clause
-                        if (!neg && !opt) sh.ldoc[slot] = kNoMoreDocs;
+                        if (!neg && !opt && !grp) sh.ldoc[slot] = kNoMoreDocs;
                     }
                 }
                 uint32_t pend_mask = __ballot_sync(0xffffffffu, pending);
@@ -921,10 +1106,13 @@ __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_
                             if (opt) {  // DisjunctionSumScorer::score_sum: clause order, from 0.0f
                                 const float o = sh.oscore[slot];
                                 sh.oscore[slot] = __fadd_rn(__float_as_uint(o) == kSent ? 0.0f : o, sc);
+                            } else if (grp) {  // the group's own DisjunctionSumScorer: member order, from 0.0f
+                                const float o = shn.gsum[slot];
+                                shn.gsum[slot] = __fadd_rn(__float_as_uint(o) == kSent ? 0.0f : o, sc);
                             } else {
                                 sh.lscore[slot] = __fadd_rn(sh.lscore[slot], sc);
                             }
-                        } else if (!neg && !opt) {
+                        } else if (!neg && !opt && !grp) {
                             sh.ldoc[slot] = kNoMoreDocs;
                         }
                         pending = false;
@@ -934,6 +1122,26 @@ __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_
                 }
             }
             __syncwarp();
+            if (GROUPS && (shn.grp[t] & 2048u)) {
+                // after a group's last member: a required group drops a slot none of its members matched and adds
+                // its sum (one f32 value) to the conjunction's; an optional one adds its sum to the optional side's
+                const bool greq = (shn.grp[t] & 512u) != 0;
+#pragma unroll
+                for (int r = 0; r < kAndSteps; r++) {
+                    const int slot = warp * kBlock + r * 32 + lane;
+                    const float g = shn.gsum[slot];
+                    shn.gsum[slot] = __uint_as_float(kSent);
+                    if (sh.ldoc[slot] == kNoMoreDocs) continue;
+                    if (greq) {
+                        if (__float_as_uint(g) == kSent) sh.ldoc[slot] = kNoMoreDocs;
+                        else sh.lscore[slot] = __fadd_rn(sh.lscore[slot], g);
+                    } else if (__float_as_uint(g) != kSent) {
+                        const float o = sh.oscore[slot];
+                        sh.oscore[slot] = __fadd_rn(__float_as_uint(o) == kSent ? 0.0f : o, g);
+                    }
+                }
+                __syncwarp();
+            }
         }
         // ---- 2b. ReqOptScorer::score over this step's collected docs, in docid order
         if (REQOPT) {
@@ -986,6 +1194,13 @@ __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_
     if (RANGES && range_lead && lane == 0)
         for (int i = 0; i < 3; i++)
             if (rstat[i]) atomicAdd(rp.blk_stats + i, rstat[i]);
+    if (GROUPS && group_lead) {
+        for (int i = 0; i < 2; i++) {
+            const unsigned long long v = __reduce_add_sync(0xffffffffu, (uint32_t)gstat[i]);
+            if (lane == 0 && v) atomicAdd(gstats + 1 + i, v);
+        }
+        if (threadIdx.x == 0) atomicAdd(gstats, 1ull);
+    }
 }
 
 template <bool REQOPT, bool OTHER>
@@ -998,6 +1213,12 @@ template <bool REQOPT, bool OTHER>
 __global__ void __launch_bounds__(kEvalThreads, OTHER ? (REQOPT ? 4 : 5) : 0)
 k_eval_and_ranges(EvalParams p, const uint32_t* __restrict__ item_ids, RangeParams rp) {
     eval_and_body<REQOPT, OTHER, true>(p, item_ids, rp);
+}
+
+template <bool REQOPT, bool OTHER>
+__global__ void __launch_bounds__(kEvalThreads, OTHER ? (REQOPT ? 4 : 5) : 0)
+k_eval_and_nested(EvalParams p, const uint32_t* __restrict__ item_ids, RangeParams rp, unsigned long long* gstats) {
+    eval_and_body<REQOPT, OTHER, true, true>(p, item_ids, rp, gstats);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1395,6 +1616,21 @@ void launch_eval_and_ranges(cudaStream_t st, const EvalParams& p, const RangePar
     else if (req_opt) launch_eval_and_ranges_t<true, false>(st, p, rp, item_ids, n);
     else if (has_other_enc) launch_eval_and_ranges_t<false, true>(st, p, rp, item_ids, n);
     else launch_eval_and_ranges_t<false, false>(st, p, rp, item_ids, n);
+}
+template <bool REQOPT, bool OTHER>
+static void launch_eval_and_nested_t(cudaStream_t st, const EvalParams& p, const RangeParams& rp,
+                                     unsigned long long* gstats, const uint32_t* item_ids, uint32_t n) {
+    cudaFuncSetAttribute(k_eval_and_nested<REQOPT, OTHER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                         (int)sizeof(AndSharedN));
+    k_eval_and_nested<REQOPT, OTHER><<<n, kEvalThreads, sizeof(AndSharedN), st>>>(p, item_ids, rp, gstats);
+}
+void launch_eval_and_nested(cudaStream_t st, const EvalParams& p, const RangeParams& rp, unsigned long long* gstats,
+                            const uint32_t* item_ids, uint32_t n, bool req_opt, bool has_other_enc) {
+    if (!n) return;
+    if (req_opt && has_other_enc) launch_eval_and_nested_t<true, true>(st, p, rp, gstats, item_ids, n);
+    else if (req_opt) launch_eval_and_nested_t<true, false>(st, p, rp, gstats, item_ids, n);
+    else if (has_other_enc) launch_eval_and_nested_t<false, true>(st, p, rp, gstats, item_ids, n);
+    else launch_eval_and_nested_t<false, false>(st, p, rp, gstats, item_ids, n);
 }
 void launch_heap_replay(cudaStream_t st, const ReplayParams& p) {
     if (!p.n_groups) return;

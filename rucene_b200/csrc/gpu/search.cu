@@ -87,6 +87,10 @@ struct rg_batch {
     Span<uint32_t> and_rng_ids, ro_rng_ids;
     uint32_t n_and_rng = 0, n_ro_rng = 0;
     Span<unsigned long long> range_stats;
+    // nested groups: the items of k_eval_and_nested and its group-lead counters (zeroed per run)
+    Span<uint32_t> and_grp_ids, ro_grp_ids;
+    uint32_t n_and_grp = 0, n_ro_grp = 0;
+    Span<unsigned long long> group_stats;
     ~rg_batch() {
         for (cudaEvent_t x : {uploaded, done, ev[0], ev[1], ev[2], ev[3]})
             if (x) cudaEventDestroy(x);
@@ -121,6 +125,7 @@ struct HostPlan {
     // point ranges: RangeRef per (leaf, range); conjunction / ReqOpt items with a range clause (k_eval_and_ranges)
     std::vector<RangeRef> range_refs;
     std::vector<uint32_t> and_rng_ids, ro_rng_ids;
+    std::vector<uint32_t> and_grp_ids, ro_grp_ids;  // conjunction / ReqOpt items with a group (k_eval_and_nested)
     // batch-local scored lists: build jobs whose dst is an offset (in floats) into the batch's list region, and the
     // col_refs entries to point there once the slab exists
     std::vector<ColumnJob> local_jobs;
@@ -142,7 +147,7 @@ struct HostPlan {
     void reset() {
         items.clear(); clauses.clear(); or_ids.clear(); ms_ids.clear(); and_ids.clear(); ro_ids.clear(); dpq_ids.clear();
         lean_ids.clear(); lean_rank.clear(); local_jobs.clear(); local_refs.clear();
-        range_refs.clear(); and_rng_ids.clear(); ro_rng_ids.clear();
+        range_refs.clear(); and_rng_ids.clear(); ro_rng_ids.clear(); and_grp_ids.clear(); ro_grp_ids.clear();
         local_floats = 0;
         local_units = 0;
         col_refs.clear(); bitmap_refs.clear(); cols.clear(); lists.clear(); or_rank.clear(); ms_rank.clear(); and_rank.clear();
@@ -172,10 +177,30 @@ struct QShape {
     // point ranges (RG_CLAUSE_RANGE, only from the *_ranges entry points): required (MUST / FILTER, or the one clause
     // a query collapses to) and MUST_NOT ones.  A shape with ranges is always kTypeAnd or kTypeReqOpt.
     std::vector<uint32_t> req_rng, not_rng;
+    // nested groups (RG_CLAUSE_GROUP, only from the *_nested entry points) of a conjunction / ReqOpt shape: the
+    // required side (MUST then FILTER) and the optional side in clause order, terms and groups mixed.  clause_idx /
+    // opt_idx still list the terms among them (columns are chosen from those); not_idx holds MUST_NOT groups flattened.
+    struct Entry {
+        bool group;
+        uint32_t ci;        // a term: its clause
+        uint32_t begin, n;  // a group: member clauses [begin, begin + n)
+        bool filter;        // a FILTER group: needs_scores = false, it scores exactly 0.0f
+    };
+    bool nested = false;
+    std::vector<Entry> req_seq, opt_seq;
 };
 
 inline bool is_range_clause(const rg_clause& c, const rg_point_range* ranges) {
     return ranges && (c.occur & RG_CLAUSE_RANGE);
+}
+
+void check_range_clause(const rg_clause& c, const rg_point_range* ranges, uint32_t n_ranges) {
+    if (c.term_id >= n_ranges) throw ArgError("range clause: term_id outside the range array");
+    const rg_point_range& r = ranges[c.term_id];
+    if (r.bytes_per_dim != 4 && r.bytes_per_dim != 8) throw ArgError("range: bytes_per_dim must be 4 or 8");
+    uint32_t wbits;
+    memcpy(&wbits, &c.weight, 4);
+    if (wbits != 0u) throw Unsupported("a boosted PointRangeQuery (weight != +0.0f)");
 }
 
 // BooleanQuery::build with PointRangeQuery clauses.  A PointRangeWeight scores 0f32 (its weight is only set by
@@ -191,12 +216,7 @@ bool classify_ranges(const rg_query& q, const rg_clause* clauses, const rg_point
         const rg_clause& c = clauses[q.clause_begin + i];
         if (!is_range_clause(c, ranges)) continue;
         any = true;
-        if (c.term_id >= n_ranges) throw ArgError("range clause: term_id outside the range array");
-        const rg_point_range& r = ranges[c.term_id];
-        if (r.bytes_per_dim != 4 && r.bytes_per_dim != 8) throw ArgError("range: bytes_per_dim must be 4 or 8");
-        uint32_t wbits;
-        memcpy(&wbits, &c.weight, 4);
-        if (wbits != 0u) throw Unsupported("a boosted PointRangeQuery (weight != +0.0f)");
+        check_range_clause(c, ranges, n_ranges);
     }
     if (!any) return false;
     if (q.flags & RG_Q_DISMAX) throw Unsupported("a PointRangeQuery in a DisjunctionMaxQuery");
@@ -331,6 +351,152 @@ QShape classify(const rg_query& q, const rg_clause* clauses, uint32_t n_clauses_
     s.msm = msm > 1 ? (uint32_t)msm : 0u;
     if (s.msm > 15u && !rescore) throw Unsupported("min_should_match > 15");
     return s;
+}
+
+// BooleanQuery::build with groups: pure-SHOULD BooleanQuerys of TermQuerys as clauses (RG_CLAUSE_GROUP).  `ext` is
+// the planner's copy of the clause array; clauses the collapses make (a one-member group as its term under the
+// group's occur, a lone FILTER group's members as FILTER terms) are appended to it.  Returns false when the query has
+// no group clause.
+//   - A group of one clause is that clause (build, :66-75); a query whose only positive clause is a group and that has
+//     no MUST_NOT clause is the group: a disjunction.  `+(a | b) -c` is ReqNotScorer(DSS(a, b), c), the tree of the
+//     disjunction `a b -c`, and runs there too.
+//   - MUST_NOT groups are flattened into MUST_NOT terms: ReqNotScorer only calls advance() and doc_id() on its
+//     excluded side (req_not_scorer.rs:46-118), and a DisjunctionSumScorer's advance() never looks at
+//     min_should_match (disjunction_scorer.rs:350-364), so excluding (a | b) is excluding a and excluding b.
+//   - Everything else needs a MUST / FILTER clause: a conjunction, or the required side of a ReqOptScorer.
+bool classify_groups(const rg_query& q, std::vector<rg_clause>& ext, uint32_t n_clauses, const rg_point_range* ranges,
+                     uint32_t n_ranges, const rg_query* groups, uint32_t n_groups, uint32_t n_caches, QShape& s) {
+    bool any = false;
+    for (uint32_t i = 0; i < q.n_clauses; i++) any = any || (ext[q.clause_begin + i].occur & RG_CLAUSE_GROUP) != 0;
+    if (!any) return false;
+    if (q.flags & RG_Q_DISMAX) throw Unsupported("a group in a DisjunctionMaxQuery");
+    if (!(q.flags & RG_Q_BOOLEAN) && q.n_clauses != 1) throw ArgError("a bare query has exactly one clause");
+    // member ranges: inside the array, apart from the query's own clauses and from the query's other groups
+    std::vector<std::pair<uint32_t, uint32_t>> spans{{q.clause_begin, q.clause_begin + q.n_clauses}};
+    std::vector<uint32_t> seen;
+    for (uint32_t i = 0; i < q.n_clauses; i++) {
+        const rg_clause& c = ext[q.clause_begin + i];
+        if (!(c.occur & RG_CLAUSE_GROUP)) continue;
+        if (c.occur & RG_CLAUSE_RANGE) throw ArgError("unknown occur");
+        if (c.term_id >= n_groups) throw ArgError("group clause: term_id outside the group array");
+        if (std::find(seen.begin(), seen.end(), c.term_id) != seen.end()) continue;
+        seen.push_back(c.term_id);
+        const rg_query& g = groups[c.term_id];
+        if ((uint64_t)g.clause_begin + g.n_clauses > n_clauses) throw ArgError("group clause range out of bounds");
+        for (const auto& sp : spans)
+            if (g.clause_begin < sp.second && sp.first < g.clause_begin + g.n_clauses)
+                throw ArgError("group clause range overlaps the query's clauses or another group");
+        spans.emplace_back(g.clause_begin, g.clause_begin + g.n_clauses);
+        if (g.flags & RG_Q_DISMAX) throw Unsupported("a DisjunctionMaxQuery inside a BooleanQuery");
+        if (!(g.flags & RG_Q_BOOLEAN)) throw ArgError("a group is a BooleanQuery (RG_Q_BOOLEAN)");
+        if (g.n_clauses == 0) throw ArgError("boolean query should at least contain one inner query!");
+        if (g.min_should_match > 1) throw Unsupported("a group with min_should_match > 1");
+        for (uint32_t j = 0; j < g.n_clauses; j++) {
+            const rg_clause& m = ext[g.clause_begin + j];
+            if (m.occur & RG_CLAUSE_GROUP) throw Unsupported("a group inside a group");
+            if (m.occur & RG_CLAUSE_RANGE) throw Unsupported("a PointRangeQuery inside a group");
+            if (m.occur == RG_MUST || m.occur == RG_FILTER || m.occur == RG_MUST_NOT)
+                throw Unsupported("a group member that is not a SHOULD TermQuery");
+            if (m.occur != RG_SHOULD) throw ArgError("unknown occur");
+            if (m.cache_id >= n_caches) throw ArgError("clause refers to an unset norm cache");
+        }
+    }
+    using Entry = QShape::Entry;
+    std::vector<Entry> musts, filters, shoulds;
+    std::vector<uint32_t> nots, should_rng;
+    size_t n_flat = 0;  // clauses of an item after flattening
+    for (uint32_t i = 0; i < q.n_clauses; i++) {
+        const uint32_t ci = q.clause_begin + i;
+        const rg_clause c = ext[ci];
+        const bool grp = (c.occur & RG_CLAUSE_GROUP) != 0;
+        const bool rng = !grp && ranges && (c.occur & RG_CLAUSE_RANGE);
+        const int32_t occ = c.occur & ~(RG_CLAUSE_GROUP | (rng ? RG_CLAUSE_RANGE : 0));
+        if (occ != RG_MUST && occ != RG_SHOULD && occ != RG_MUST_NOT && occ != RG_FILTER) throw ArgError("unknown occur");
+        if (rng) {
+            check_range_clause(c, ranges, n_ranges);
+            n_flat++;
+            (occ == RG_MUST_NOT ? s.not_rng : occ == RG_SHOULD ? should_rng : s.req_rng).push_back(ci);
+            continue;
+        }
+        Entry e{false, ci, 0, 0, false};
+        if (grp) {
+            const rg_query& g = groups[c.term_id];
+            if (g.n_clauses == 1) {  // a group of one clause is that clause
+                const rg_clause& m = ext[g.clause_begin];
+                e.ci = (uint32_t)ext.size();
+                ext.push_back(rg_clause{occ, m.term_id, m.weight, m.cache_id});
+            } else {
+                e = Entry{true, 0, g.clause_begin, g.n_clauses, occ == RG_FILTER};
+            }
+        }
+        n_flat += e.group ? e.n : 1;
+        if (occ == RG_MUST_NOT) {
+            if (e.group)
+                for (uint32_t j = 0; j < e.n; j++) nots.push_back(e.begin + j);
+            else nots.push_back(e.ci);
+        } else {
+            (occ == RG_MUST ? musts : occ == RG_FILTER ? filters : shoulds).push_back(e);
+        }
+    }
+    auto lone_group = [&](const Entry& e) {  // the query is the group: a disjunction of its members
+        if (e.n > (uint32_t)kDpqMaxTerms || (e.n + nots.size() > (size_t)kMaxTerms && !nots.empty()))
+            throw Unsupported("more than 9 clauses (only pure SHOULD disjunctions of up to 32 clauses go wider)");
+        s.type = kTypeOr;
+        for (uint32_t j = 0; j < e.n; j++) {
+            if (e.filter) {  // ConstantScoreQuery(.., 0) of the group: members that score 0
+                const rg_clause& m = ext[e.begin + j];
+                s.clause_idx.push_back((uint32_t)ext.size());
+                ext.push_back(rg_clause{RG_FILTER, m.term_id, 0.0f, m.cache_id});
+            } else {
+                s.clause_idx.push_back(e.begin + j);
+            }
+        }
+    };
+    const size_t n_pos = musts.size() + filters.size() + shoulds.size() + s.req_rng.size() + should_rng.size();
+    if (n_pos == 0 && !s.req_rng.empty()) throw ArgError("internal: range bookkeeping");
+    if (nots.empty() && s.not_rng.empty() && n_pos == 1) {  // collapses to the one positive clause (:66-75)
+        if (!s.req_rng.empty() || !should_rng.empty()) {
+            s.type = kTypeAnd;
+            if (s.req_rng.empty()) s.req_rng = should_rng;
+            return true;
+        }
+        const Entry& e = !musts.empty() ? musts[0] : !filters.empty() ? filters[0] : shoulds[0];
+        if (e.group) {
+            lone_group(e);
+        } else {
+            s.type = kTypeOr;
+            s.clause_idx.push_back(e.ci);
+        }
+        return true;
+    }
+    if (n_flat > (size_t)kMaxTerms) throw Unsupported("more than 9 clauses after flattening the groups");
+    if (n_pos == 0) {  // only MUST_NOT clauses: MatchAllDocsQuery beside them (:76-79)
+        if (!s.not_rng.empty()) throw Unsupported("a PointRangeQuery on a disjunction or beside only MUST_NOT clauses");
+        s.type = kTypeOr;
+        s.match_all = true;
+        s.not_idx = nots;
+        return true;
+    }
+    if (musts.empty() && filters.empty() && s.req_rng.empty())
+        throw Unsupported("a group in a disjunction (no MUST / FILTER clause)");
+    if (!should_rng.empty()) throw Unsupported("a SHOULD PointRangeQuery beside a required clause");
+    if (musts.size() == 1 && musts[0].group && filters.empty() && shoulds.empty() && s.req_rng.empty() &&
+        s.not_rng.empty()) {
+        lone_group(musts[0]);  // ReqNotScorer(DSS(members), MUST_NOT side)
+        s.not_idx = nots;
+        return true;
+    }
+    s.nested = true;
+    s.type = shoulds.empty() ? kTypeAnd : kTypeReqOpt;
+    s.req_seq = musts;
+    s.req_seq.insert(s.req_seq.end(), filters.begin(), filters.end());
+    s.opt_seq = shoulds;
+    for (const Entry& e : s.req_seq)
+        if (!e.group) s.clause_idx.push_back(e.ci);
+    for (const Entry& e : s.opt_seq)
+        if (!e.group) s.opt_idx.push_back(e.ci);
+    s.not_idx = nots;
+    return true;
 }
 
 // BooleanWeight::create_scorer / DisjunctionMaxWeight::create_scorer for one (query, leaf): which clauses of the
@@ -963,16 +1129,25 @@ void choose_local_lists(rg_engine* e, const std::vector<QShape>& shapes, const r
 
 void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
                 uint32_t n_clauses, uint32_t mode, float k1, HostPlan& hp, PlanTimer& tm, PlanScratch& scratch,
-                const rg_point_range* ranges, uint32_t n_ranges) {
+                const rg_point_range* ranges, uint32_t n_ranges, const rg_query* groups = nullptr,
+                uint32_t n_groups = 0) {
     const uint32_t n_caches = (uint32_t)(e->h_caches.size() / 256);
     const uint32_t n_segs = (uint32_t)e->segs.size();
     std::vector<QShape> shapes(n_queries);
-    bool any_ranges = false;
+    bool any_ranges = false, any_groups = false;
+    // groups: the clause array grows by what the collapses make (classify_groups)
+    std::vector<rg_clause> ext;
+    if (groups) ext.assign(clauses, clauses + n_clauses);
     for (uint32_t qi = 0; qi < n_queries; qi++) {
         if (ranges && (uint64_t)queries[qi].clause_begin + queries[qi].n_clauses > n_clauses)
             throw ArgError("query clause range out of bounds");
-        if (ranges && classify_ranges(queries[qi], clauses, ranges, n_ranges, shapes[qi])) any_ranges = true;
-        else shapes[qi] = classify(queries[qi], clauses, n_clauses);
+        if (groups && classify_groups(queries[qi], ext, n_clauses, ranges, n_ranges, groups, n_groups, n_caches, shapes[qi])) {
+            any_groups = true;
+            any_ranges = any_ranges || !shapes[qi].req_rng.empty() || !shapes[qi].not_rng.empty();
+        } else if (ranges && classify_ranges(queries[qi], groups ? ext.data() : clauses, ranges, n_ranges, shapes[qi]))
+            any_ranges = true;
+        else shapes[qi] = classify(queries[qi], groups ? ext.data() : clauses, n_clauses);
+        if (groups) clauses = ext.data();  // (ext may have moved)
         for (uint32_t ci : shapes[qi].clause_idx)
             if (clauses[ci].cache_id >= n_caches) throw ArgError("clause refers to an unset norm cache");
         for (uint32_t ci : shapes[qi].opt_idx)
@@ -1053,6 +1228,139 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
             // resolve clauses against this leaf: present (conjunctions in cost order), MUST_NOT, optional side
             std::vector<uint32_t> present, nots, opts;
             const bool new_group = mode == RG_MODE_SEARCH_PARALLEL || !group_open;
+            if (shape.nested) {
+                // BooleanWeight::create_scorer with groups in this leaf: a group is a DisjunctionSumScorer over its
+                // members present here (even over one: the `1 =>` arm is commented out, boolean_query.rs:196-279),
+                // None when it has none (a required group kills the leaf, an optional one is left out); its cost()
+                // is the sum of those members' doc_freq (disjunction_scorer.rs:39).
+                auto df_of = [&](uint32_t ci) -> uint64_t {
+                    const uint32_t t = clauses[ci].term_id;
+                    return t < seg.host_terms.size() && seg.host_terms[t].doc_freq > 0 ? (uint64_t)seg.host_terms[t].doc_freq : 0;
+                };
+                struct Req { uint64_t cost; QShape::Entry e; std::vector<uint32_t> members; };
+                auto resolve = [&](const QShape::Entry& e, Req& r) {
+                    r = Req{0, e, {}};
+                    if (!e.group) return (r.cost = df_of(e.ci)) > 0;
+                    for (uint32_t j = 0; j < e.n; j++)
+                        if (const uint64_t df = df_of(e.begin + j)) {
+                            r.members.push_back(e.begin + j);
+                            r.cost += df;
+                        }
+                    return !r.members.empty();
+                };
+                std::vector<Req> req, opt;
+                bool dead = false;
+                for (const QShape::Entry& e : shape.req_seq) {
+                    Req r;
+                    if (!resolve(e, r)) dead = true;
+                    req.push_back(std::move(r));
+                }
+                if (dead) continue;
+                for (const QShape::Entry& e : shape.opt_seq) {
+                    Req r;
+                    if (resolve(e, r)) opt.push_back(std::move(r));
+                }
+                for (uint32_t ci : shape.not_idx)
+                    if (df_of(ci)) nots.push_back(ci);
+                std::vector<std::pair<uint64_t, uint32_t>> rreq;
+                std::vector<uint32_t> rnots;
+                if ((!shape.req_rng.empty() || !shape.not_rng.empty()) &&
+                    !resolve_ranges(shape, seg, clauses, ranges, rreq, rnots))
+                    continue;
+                // ConjunctionScorer::new: stable sort by cost() (:30); the score is lead1 + lead2 + the others in
+                // that order, each group one f32 value
+                std::stable_sort(req.begin(), req.end(), [](const Req& a, const Req& b) { return a.cost < b.cost; });
+                // the cheapest required clause leads (a range only when it is cheaper than every term and group)
+                const bool range_lead = !rreq.empty() && (req.empty() || rreq[0].first < req[0].cost);
+                const int leaf_type = shape.type == kTypeReqOpt && opt.empty() ? (int)kTypeAnd : shape.type;
+                const uint64_t cost = range_lead ? rreq[0].first : req[0].cost;
+                uint64_t bytes = 0;
+                for (const Req& r : req) {
+                    if (!r.e.group) bytes += seg.host_terms[clauses[r.e.ci].term_id].enc_bytes;
+                    for (uint32_t ci : r.members) bytes += seg.host_terms[clauses[ci].term_id].enc_bytes;
+                }
+                lp.postings += cost;
+                lp.algo_bytes += bytes + cost;
+                const uint32_t clause_begin = (uint32_t)lp.clauses.size();
+                auto col_of = [&](uint32_t ci) -> int64_t {
+                    if (columns.empty()) return -1;
+                    const rg_clause& c = clauses[ci];
+                    const float w = clause_weight(c);
+                    uint32_t wbits;
+                    memcpy(&wbits, &w, 4);
+                    const auto it = columns.find(ColKey(si, c.term_id, wbits, c.cache_id, k1bits));
+                    return it == columns.end() ? -1 : (int64_t)it->second;
+                };
+                auto range_clause = [&](uint32_t ci, uint32_t not_flag) {
+                    return ItemClause{si * n_ranges + clauses[ci].term_id, 0.0f, 0u, 256u | not_flag};
+                };
+                // a group's members are contiguous, in member order, and always block streams (a group that leads is
+                // merged from its members' blocks); bit9 / bit10: member of a required / optional group, bit11: last
+                auto put = [&](const Req& r, bool lead, uint32_t side) {
+                    if (r.e.group) {
+                        for (size_t j = 0; j < r.members.size(); j++) {
+                            const rg_clause& m = clauses[r.members[j]];
+                            const uint32_t last = j + 1 == r.members.size() ? 2048u : 0u;
+                            lp.clauses.push_back(ItemClause{m.term_id, r.e.filter ? 0.0f : m.weight, m.cache_id,
+                                                            (side == 2u ? 1024u : 512u) | last});
+                        }
+                        return;
+                    }
+                    const rg_clause& c = clauses[r.e.ci];
+                    const float w = side == 2u ? c.weight : clause_weight(c);
+                    const int64_t col = lead ? -1 : col_of(r.e.ci);
+                    if (col >= 0) lp.clauses.push_back(ItemClause{(uint32_t)col, w, c.cache_id, side | 4u});
+                    else lp.clauses.push_back(ItemClause{c.term_id, w, c.cache_id, side});
+                };
+                if (range_lead) lp.clauses.push_back(range_clause(rreq[0].second, 0u));
+                for (size_t i = 0; i < req.size(); i++) put(req[i], i == 0 && !range_lead, 0u);
+                for (size_t i = range_lead ? 1 : 0; i < rreq.size(); i++) lp.clauses.push_back(range_clause(rreq[i].second, 0u));
+                for (uint32_t ci : nots) {
+                    const int64_t col = col_of(ci);
+                    if (col >= 0) lp.clauses.push_back(ItemClause{(uint32_t)col, 0.0f, clauses[ci].cache_id, 1u | 4u});
+                    else lp.clauses.push_back(ItemClause{clauses[ci].term_id, 0.0f, clauses[ci].cache_id, 1u});
+                }
+                for (uint32_t ci : rnots) lp.clauses.push_back(range_clause(ci, 1u));
+                for (const Req& r : opt) put(r, false, 2u);
+                const uint32_t n_item_terms = (uint32_t)(lp.clauses.size() - clause_begin);
+                if (n_item_terms > (uint32_t)kMaxTerms || (!range_lead && req[0].members.size() > 8u))  // a leading group: one warp of k_eval_and_nested per member
+                    throw Unsupported("a nested item wider than k_eval_and_nested takes");  // (n_flat <= 9 keeps this unreachable)
+                // docid ranges as for a conjunction; a ReqOptScorer with a required term or group keeps its running
+                // mean over the whole leaf
+                uint64_t R = std::min<uint64_t>((cost + and_rp - 1) / and_rp, max_ranges);
+                R = std::max<uint64_t>(1, std::min<uint64_t>(R, (uint64_t)(seg.max_doc + kBlock - 1) / kBlock));
+                if (leaf_type == (int)kTypeReqOpt && !req.empty()) R = 1;
+                const uint64_t n_lead_blocks = (uint64_t)(seg.max_doc + kBlock - 1) / kBlock;
+                if (new_group) {
+                    lp.group_out.push_back(mode == RG_MODE_SEARCH_PARALLEL ? si * n_queries + qi : qi);
+                    group_open = true;
+                }
+                for (uint64_t r = 0; r < R; r++) {
+                    WorkItem it{};
+                    it.query = qi;
+                    it.seg = (uint16_t)si;
+                    it.type = (uint8_t)leaf_type;
+                    it.n_terms = (uint8_t)n_item_terms;
+                    it.lo = (int32_t)((uint64_t)seg.max_doc * r / R);
+                    it.hi = (int32_t)((uint64_t)seg.max_doc * (r + 1) / R);
+                    if (range_lead) {
+                        it.lo = (int32_t)(n_lead_blocks * r / R * kBlock);
+                        it.hi = r + 1 == R ? seg.max_doc : (int32_t)(n_lead_blocks * (r + 1) / R * kBlock);
+                    }
+                    it.clause_begin = clause_begin;
+                    it.chain_pos = (r == 0 && new_group) ? 0u : chain_pos;
+                    chain_pos = it.chain_pos + 1;
+                    const uint32_t idx = (uint32_t)lp.items.size();
+                    lp.items.push_back(it);
+                    if (leaf_type == (int)kTypeReqOpt) {
+                        lp.ro_ids.push_back(idx);
+                    } else {
+                        lp.and_ids.push_back(idx);
+                        lp.and_rank.push_back((uint32_t)r);
+                    }
+                }
+                continue;
+            }
             if (!resolve_leaf(shape, seg, clauses, present, nots, opts)) continue;
             // point ranges: the required ones with their point counts (cheapest first) and the MUST_NOT ones
             std::vector<std::pair<uint64_t, uint32_t>> rreq;
@@ -1381,19 +1689,23 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
     by_rank(hp.ms_ids, hp.ms_rank);
     by_rank(hp.lean_ids, hp.lean_rank);
     by_rank(hp.and_ids, hp.and_rank);
+    auto split = [&](std::vector<uint32_t>& ids, std::vector<uint32_t>& out_ids, uint32_t flags) {
+        std::vector<uint32_t> keep;
+        for (uint32_t id : ids) {
+            const WorkItem& it = hp.items[id];
+            bool r = false;
+            for (uint32_t c = 0; c < it.n_terms; c++) r = r || (hp.clauses[it.clause_begin + c].flags & flags) != 0;
+            (r ? out_ids : keep).push_back(id);
+        }
+        ids.swap(keep);
+    };
+    if (any_groups) {  // items with a group go to k_eval_and_nested (ranges or not), in the same launch order
+        split(hp.and_ids, hp.and_grp_ids, 512u | 1024u);
+        split(hp.ro_ids, hp.ro_grp_ids, 512u | 1024u);
+    }
     if (any_ranges) {  // items with a range clause go to k_eval_and_ranges, in the same launch order
-        auto split = [&](std::vector<uint32_t>& ids, std::vector<uint32_t>& rng_ids) {
-            std::vector<uint32_t> keep;
-            for (uint32_t id : ids) {
-                const WorkItem& it = hp.items[id];
-                bool r = false;
-                for (uint32_t c = 0; c < it.n_terms; c++) r = r || (hp.clauses[it.clause_begin + c].flags & 256u) != 0;
-                (r ? rng_ids : keep).push_back(id);
-            }
-            ids.swap(keep);
-        };
-        split(hp.and_ids, hp.and_rng_ids);
-        split(hp.ro_ids, hp.ro_rng_ids);
+        split(hp.and_ids, hp.and_rng_ids, 256u);
+        split(hp.ro_ids, hp.ro_rng_ids, 256u);
     }
     // heap groups = contiguous item runs starting at chain-start items
     for (uint32_t i = 0; i < hp.items.size(); i++)
@@ -1529,7 +1841,7 @@ extern "C" {
 
 static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
                          uint32_t n_clauses, const rg_search_params* p, const rg_point_range* ranges, uint32_t n_ranges,
-                         rg_batch** out) {
+                         rg_batch** out, const rg_query* groups = nullptr, uint32_t n_groups = 0) {
     RG_TRY
     if (!e || !p || !out || (n_queries && !queries) || (n_clauses && !clauses)) throw ArgError("null argument");
     *out = nullptr;
@@ -1546,7 +1858,8 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
     PlanScratch& scratch = *static_cast<PlanScratch*>(e->plan_scratch.get());
     HostPlan& hp = scratch.hp;
     hp.reset();
-    plan_batch(e, queries, n_queries, clauses, n_clauses, p->mode, p->k1, hp, tm, scratch, ranges, n_ranges);
+    plan_batch(e, queries, n_queries, clauses, n_clauses, p->mode, p->k1, hp, tm, scratch, ranges, n_ranges, groups,
+               n_groups);
     std::unique_ptr<rg_batch> b(new rg_batch());
     b->generation = e->generation;
     b->cols = std::move(hp.cols);
@@ -1571,6 +1884,8 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
     b->n_ro = (uint32_t)hp.ro_ids.size();
     b->n_and_rng = (uint32_t)hp.and_rng_ids.size();
     b->n_ro_rng = (uint32_t)hp.ro_rng_ids.size();
+    b->n_and_grp = (uint32_t)hp.and_grp_ids.size();
+    b->n_ro_grp = (uint32_t)hp.ro_grp_ids.size();
     b->n_groups = (uint32_t)hp.group_out.size();
     b->max_or_terms = hp.max_or_terms;
     b->or_has_not = hp.or_has_not;
@@ -1605,6 +1920,8 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
     carve(b->range_refs, hp.range_refs.size());
     carve(b->and_rng_ids, hp.and_rng_ids.size());
     carve(b->ro_rng_ids, hp.ro_rng_ids.size());
+    carve(b->and_grp_ids, hp.and_grp_ids.size());
+    carve(b->ro_grp_ids, hp.ro_grp_ids.size());
     // running top-k scores of every OR work item (theta inheritance along a heap chain); skipped when it would
     // not fit comfortably (huge batches with k near 1024): theta then falls back to the per-range bound
     b->topk_cap = (std::min<uint32_t>(p->k, 1024u) + 31u) & ~31u;
@@ -1619,6 +1936,7 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
     carve(b->arena_next, 2);
     carve(b->dbg, 16);
     carve(b->range_stats, 3);
+    carve(b->group_stats, 3);
     carve(b->out_hits, (size_t)std::max<uint32_t>(1, n_queries) * p->k);
     carve(b->out_counts, n_queries);
     carve(b->out_total, n_queries);
@@ -1651,6 +1969,7 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
     rebase(b->item_theta); rebase(b->item_topk_n); rebase(b->item_topk); rebase(b->arena_next); rebase(b->dbg); rebase(b->out_hits); rebase(b->out_counts);
     rebase(b->out_total);
     rebase(b->range_refs); rebase(b->and_rng_ids); rebase(b->ro_rng_ids); rebase(b->range_stats);
+    rebase(b->and_grp_ids); rebase(b->ro_grp_ids); rebase(b->group_stats);
     if (p->mode == RG_MODE_SEARCH_PARALLEL) rebase(b->leaf_records);
     b->zero_begin = b->slab.p + zero_off;
     b->zero_bytes = off - zero_off;
@@ -1671,6 +1990,8 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
     up(b->range_refs, hp.range_refs, cs);
     up(b->and_rng_ids, hp.and_rng_ids, cs);
     up(b->ro_rng_ids, hp.ro_rng_ids, cs);
+    up(b->and_grp_ids, hp.and_grp_ids, cs);
+    up(b->ro_grp_ids, hp.ro_grp_ids, cs);
     RG_CUDA_CHECK(cudaEventCreateWithFlags(&b->uploaded, cudaEventDisableTiming));
     RG_CUDA_CHECK(cudaEventCreateWithFlags(&b->done, cudaEventDisableTiming));
     for (auto& x : b->ev) RG_CUDA_CHECK(cudaEventCreate(&x));
@@ -1692,9 +2013,10 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
     b->h2d_bytes = (hp.items.size() * sizeof(WorkItem)) + hp.clauses.size() * sizeof(ItemClause) +
                    4 * (hp.or_ids.size() + hp.lean_ids.size() + hp.ms_ids.size() + hp.dpq_ids.size() + hp.and_ids.size() + hp.ro_ids.size() + hp.group_item_begin.size() + hp.group_out.size()) +
                    hp.col_refs.size() * sizeof(ColRef) + hp.range_refs.size() * sizeof(RangeRef) +
-                   4 * (hp.and_rng_ids.size() + hp.ro_rng_ids.size());
+                   4 * (hp.and_rng_ids.size() + hp.ro_rng_ids.size() + hp.and_grp_ids.size() + hp.ro_grp_ids.size());
     b->kernels_per_run = (b->n_lean ? 1 : 0) + (b->n_ms ? 1 : 0) + (b->n_dpq ? 1 : 0) + (b->n_or ? 1 : 0) + (b->n_and ? 1 : 0) + (b->n_ro ? 1 : 0) + (b->n_groups ? 1 : 0) +
-                         (p->mode == RG_MODE_SEARCH_PARALLEL ? 1 : 0) + (b->n_and_rng ? 1 : 0) + (b->n_ro_rng ? 1 : 0);
+                         (p->mode == RG_MODE_SEARCH_PARALLEL ? 1 : 0) + (b->n_and_rng ? 1 : 0) + (b->n_ro_rng ? 1 : 0) +
+                         (b->n_and_grp ? 1 : 0) + (b->n_ro_grp ? 1 : 0);
     tm.mark("alloc_copy_issue");
     RG_CUDA_CHECK(cudaStreamSynchronize(cs));  // the host vectors go out of scope (a running batch is not waited for)
     tm.mark("sync");
@@ -1720,6 +2042,21 @@ int rg_batch_prepare_ranges(rg_engine* e, const rg_query* queries, uint32_t n_qu
     // a non-null array (even of length 0) makes range clauses readable
     static const rg_point_range none{};
     return batch_prepare(e, queries, n_queries, clauses, n_clauses, p, ranges ? ranges : &none, n_ranges, out);
+}
+
+int rg_batch_prepare_nested(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                            uint32_t n_clauses, const rg_search_params* p, const rg_point_range* ranges,
+                            uint32_t n_ranges, const rg_query* groups, uint32_t n_groups, rg_batch** out) {
+    if ((n_ranges && !ranges) || (n_groups && !groups)) {
+        if (out) *out = nullptr;
+        g_last_error = "null argument";
+        return RG_EINVAL;
+    }
+    // non-null arrays (even of length 0) make range and group clauses readable
+    static const rg_point_range none{};
+    static const rg_query no_group{};
+    return batch_prepare(e, queries, n_queries, clauses, n_clauses, p, ranges ? ranges : &none, n_ranges, out,
+                         groups ? groups : &no_group, n_groups);
 }
 
 int rg_batch_run(rg_engine* e, rg_batch* b) {
@@ -1776,6 +2113,10 @@ int rg_batch_run(rg_engine* e, rg_batch* b) {
     launch_eval_and_ranges(st, ep, rgp, b->and_rng_ids.p, b->n_and_rng, false, has_other);
     RG_CUDA_CHECK(cudaGetLastError());
     launch_eval_and_ranges(st, ep, rgp, b->ro_rng_ids.p, b->n_ro_rng, true, has_other);
+    RG_CUDA_CHECK(cudaGetLastError());
+    launch_eval_and_nested(st, ep, rgp, b->group_stats.p, b->and_grp_ids.p, b->n_and_grp, false, has_other);
+    RG_CUDA_CHECK(cudaGetLastError());
+    launch_eval_and_nested(st, ep, rgp, b->group_stats.p, b->ro_grp_ids.p, b->n_ro_grp, true, has_other);
     RG_CUDA_CHECK(cudaGetLastError());
     RG_CUDA_CHECK(cudaEventRecord(b->ev[3], st));
     ReplayParams rp{};
@@ -1908,6 +2249,26 @@ int rg_search_batch_ranges(rg_engine* e, const rg_query* queries, uint32_t n_que
     return rc;
 }
 
+int rg_search_batch_nested(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                           uint32_t n_clauses, const rg_search_params* p, const rg_point_range* ranges,
+                           uint32_t n_ranges, const rg_query* groups, uint32_t n_groups, rg_hit* out_hits,
+                           uint32_t* out_counts, uint64_t* out_total_hits) {
+    rg_batch* b = nullptr;
+    int rc = rg_batch_prepare_nested(e, queries, n_queries, clauses, n_clauses, p, ranges, n_ranges, groups, n_groups, &b);
+    if (rc != RG_OK) return rc;
+    rc = rg_batch_run(e, b);
+    if (rc == RG_OK) rc = rg_batch_fetch(e, b, out_hits, out_counts, out_total_hits);
+    rg_batch_destroy(e, b);
+    if (rc == RG_ENOMEM && n_queries > 1 && p && p->k) {  // as rg_search_batch
+        const uint32_t h = n_queries / 2;
+        rc = rg_search_batch_nested(e, queries, h, clauses, n_clauses, p, ranges, n_ranges, groups, n_groups, out_hits,
+                                    out_counts, out_total_hits);
+        if (rc == RG_OK)
+            rc = rg_search_batch_nested(e, queries + h, n_queries - h, clauses, n_clauses, p, ranges, n_ranges, groups,
+                                        n_groups, out_hits + (size_t)h * p->k, out_counts + h, out_total_hits + h);
+    }
+    return rc;
+}
 int rg_batch_range_stats(rg_engine* e, rg_batch* b, uint64_t out[3]) {
     RG_TRY
     if (!e || !b || !out) throw ArgError("null argument");
@@ -1915,6 +2276,18 @@ int rg_batch_range_stats(rg_engine* e, rg_batch* b, uint64_t out[3]) {
     if (b->ran) {
         RG_CUDA_CHECK(cudaStreamSynchronize(e->stream));
         RG_CUDA_CHECK(cudaMemcpy(out, b->range_stats.p, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    }
+    return RG_OK;
+    RG_CATCH
+}
+
+int rg_batch_group_stats(rg_engine* e, rg_batch* b, uint64_t out[3]) {
+    RG_TRY
+    if (!e || !b || !out) throw ArgError("null argument");
+    memset(out, 0, 3 * sizeof(uint64_t));
+    if (b->ran) {
+        RG_CUDA_CHECK(cudaStreamSynchronize(e->stream));
+        RG_CUDA_CHECK(cudaMemcpy(out, b->group_stats.p, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
     }
     return RG_OK;
     RG_CATCH

@@ -241,13 +241,18 @@ public:
     void search(const Query& query, TopDocsCollector& collector) {
         std::vector<rg_clause> clauses;
         std::vector<rg_point_range> ranges;
-        rg_query q = compile(query, clauses, &ranges);
+        std::vector<rg_query> groups;
+        rg_query q = compile(query, clauses, &ranges, &groups);
         const uint32_t k = (uint32_t)collector.estimated_hits();
         std::vector<rg_hit> hits(k);
         uint32_t count = 0;
         uint64_t total = 0;
         rg_search_params p{k, sim_.k1, RG_MODE_SEARCH, 0};
-        if (ranges.empty())
+        if (!groups.empty())
+            check(rg_search_batch_nested(engine_, &q, 1, clauses.data(), (uint32_t)clauses.size(), &p, ranges.data(),
+                                         (uint32_t)ranges.size(), groups.data(), (uint32_t)groups.size(), hits.data(),
+                                         &count, &total));
+        else if (ranges.empty())
             check(rg_search_batch(engine_, &q, 1, clauses.data(), (uint32_t)clauses.size(), &p, hits.data(), &count, &total));
         else
             check(rg_search_batch_ranges(engine_, &q, 1, clauses.data(), (uint32_t)clauses.size(), &p, ranges.data(),
@@ -302,11 +307,23 @@ private:
         c.cache_id = 0;
         return c;
     }
-    // a TermQuery or (ranges != null) a PointRangeQuery as one clause
+    using Pending = std::vector<std::pair<size_t, const BooleanQuery*>>;  // (group index, nested query)
+    // a TermQuery, (ranges != null) a PointRangeQuery or (groups != null) a nested pure-SHOULD BooleanQuery of
+    // TermQuerys as one clause; a group's members are written after the query's own clauses (compile)
     void add_clause(const Query& leaf, int32_t occur, std::vector<rg_clause>& clauses,
-                    std::vector<rg_point_range>* ranges) const {
+                    std::vector<rg_point_range>* ranges, std::vector<rg_query>* groups = nullptr,
+                    Pending* pending = nullptr) const {
         if (auto tq = dynamic_cast<const TermQuery*>(&leaf)) {
             clauses.push_back(clause_of(*tq, occur));
+            return;
+        }
+        if (auto bq = dynamic_cast<const BooleanQuery*>(&leaf); bq && groups) {
+            bool pure = bq->must_queries.empty() && bq->filter_queries.empty() && bq->must_not_queries.empty();
+            for (const QueryPtr& m : bq->should_queries) pure = pure && dynamic_cast<const TermQuery*>(m.get());
+            if (!pure) throw UnsupportedQuery("only pure-SHOULD groups of TermQuerys are accelerated");
+            clauses.push_back(rg_clause{occur | RG_CLAUSE_GROUP, (uint32_t)groups->size(), 0.0f, 0u});
+            pending->emplace_back(groups->size(), bq);
+            groups->push_back(rg_query{0u, 0u, bq->min_should_match, RG_Q_BOOLEAN});
             return;
         }
         auto pq = dynamic_cast<const PointRangeQuery*>(&leaf);
@@ -321,8 +338,21 @@ private:
         clauses.push_back(rg_clause{occur | RG_CLAUSE_RANGE, (uint32_t)ranges->size(), 0.0f, 0u});
         ranges->push_back(r);
     }
-    rg_query compile(const Query& query, std::vector<rg_clause>& clauses,
-                     std::vector<rg_point_range>* ranges = nullptr) const {
+    rg_query compile(const Query& query, std::vector<rg_clause>& clauses, std::vector<rg_point_range>* ranges = nullptr,
+                     std::vector<rg_query>* groups = nullptr) const {
+        Pending pending;
+        const rg_query q = compile_one(query, clauses, ranges, groups, &pending);
+        for (const auto& g : pending) {
+            rg_query& gq = (*groups)[g.first];
+            gq.clause_begin = (uint32_t)clauses.size();
+            gq.n_clauses = (uint32_t)g.second->should_queries.size();
+            for (const QueryPtr& m : g.second->should_queries)
+                clauses.push_back(clause_of(static_cast<const TermQuery&>(*m), RG_SHOULD));
+        }
+        return q;
+    }
+    rg_query compile_one(const Query& query, std::vector<rg_clause>& clauses, std::vector<rg_point_range>* ranges,
+                         std::vector<rg_query>* groups, Pending* pending) const {
         rg_query q{};
         q.clause_begin = (uint32_t)clauses.size();
         if (dynamic_cast<const TermQuery*>(&query) || dynamic_cast<const PointRangeQuery*>(&query)) {
@@ -332,7 +362,7 @@ private:
         }
         if (auto cq = dynamic_cast<const ConstantScoreQuery*>(&query)) {  // the lone FILTER clause of build()
             if (!cq->query || cq->boost != 0.0f) throw UnsupportedQuery("only ConstantScoreQuery(leaf, 0) is accelerated");
-            add_clause(*cq->query, RG_FILTER, clauses, ranges);
+            add_clause(*cq->query, RG_FILTER, clauses, ranges, groups, pending);
             q.n_clauses = 1;
             q.flags = RG_Q_BOOLEAN;
             return q;
@@ -344,7 +374,7 @@ private:
             bq->filter_queries.empty() && !bq->must_not_queries.empty())
             musts.clear();  // the engine reads "only MUST_NOT clauses" as MatchAllDocsQuery minus those terms
         auto add = [&](const std::vector<QueryPtr>& v, int32_t occur) {
-            for (const QueryPtr& c : v) add_clause(*c, occur, clauses, ranges);
+            for (const QueryPtr& c : v) add_clause(*c, occur, clauses, ranges, groups, pending);
         };
         add(musts, RG_MUST);
         add(bq->filter_queries, RG_FILTER);

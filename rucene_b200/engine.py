@@ -27,6 +27,7 @@ CLAUSE_DTYPE = np.dtype([("occur", "<i4"), ("term_id", "<u4"), ("weight", "<f4")
 QUERY_DTYPE = np.dtype([("clause_begin", "<u4"), ("n_clauses", "<u4"),
                         ("min_should_match", "<i4"), ("flags", "<u4")])
 HIT_DTYPE = np.dtype([("doc", "<i4"), ("score", "<f4")])
+CLAUSE_GROUP = 0x200   # rg_clause.occur bit: a pure-SHOULD group of terms, term_id indexes the group array (*_nested)
 CLAUSE_RANGE = 0x100   # rg_clause.occur bit: a point-range clause, term_id indexes the range array (*_ranges calls)
 RANGE_DTYPE = np.dtype([("field", "<u4"), ("bytes_per_dim", "<u4"), ("lower", "u1", 8), ("upper", "u1", 8)])
 
@@ -97,6 +98,11 @@ def lib():
     L.rg_search_batch_ranges.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(SearchParams), vp,
                                          C.c_uint32, vp, vp, vp]
     L.rg_batch_range_stats.argtypes = [vp, vp, vp]
+    L.rg_batch_prepare_nested.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(SearchParams), vp,
+                                          C.c_uint32, vp, C.c_uint32, C.POINTER(vp)]
+    L.rg_search_batch_nested.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(SearchParams), vp,
+                                         C.c_uint32, vp, C.c_uint32, vp, vp, vp]
+    L.rg_batch_group_stats.argtypes = [vp, vp, vp]
     L.rg_batch_run.argtypes = [vp, vp]
     L.rg_batch_fetch.argtypes = [vp, vp, vp, vp, vp]
     L.rg_batch_destroy.argtypes = [vp, vp]
@@ -148,6 +154,12 @@ class Batch:
         _check(lib().rg_batch_fetch(self.engine.h, self.h, _p(hits), _p(counts), _p(total)),
                self.engine.h)
         return hits, counts, total
+
+    def group_stats(self):
+        """Group leads of the last run: items a group led, member postings merged, postings that became holes."""
+        out = np.zeros(3, np.uint64)
+        _check(lib().rg_batch_group_stats(self.engine.h, self.h, _p(out)), self.engine.h)
+        return {"items": int(out[0]), "merged": int(out[1]), "holes": int(out[2])}
 
     def range_stats(self):
         """Range-lead 128-doc blocks of the last run: skipped, taken whole, scanned."""
@@ -346,13 +358,19 @@ class Engine:
                                      _p(counts), _p(total)), self.h)
         return hits, counts, total
 
-    def prepare(self, queries, clauses, k, k1=1.2, mode=MODE_SEARCH, ranges=None):
-        """ranges (RANGE_DTYPE array, may be empty): clauses with CLAUSE_RANGE in occur are point ranges."""
+    def prepare(self, queries, clauses, k, k1=1.2, mode=MODE_SEARCH, ranges=None, groups=None):
+        """ranges (RANGE_DTYPE array, may be empty): clauses with CLAUSE_RANGE in occur are point ranges.
+        groups (QUERY_DTYPE array, may be empty): clauses with CLAUSE_GROUP in occur are pure-SHOULD groups."""
         q = np.ascontiguousarray(queries, dtype=QUERY_DTYPE)
         c = np.ascontiguousarray(clauses, dtype=CLAUSE_DTYPE)
         p = self._params(k, k1, mode)
         h = C.c_void_p()
-        if ranges is None:
+        if groups is not None:
+            g = np.ascontiguousarray(groups, dtype=QUERY_DTYPE)
+            r = None if ranges is None else np.ascontiguousarray(ranges, dtype=RANGE_DTYPE)
+            _check(lib().rg_batch_prepare_nested(self.h, _p(q), len(q), _p(c), len(c), C.byref(p), _p(r),
+                                                 0 if r is None else len(r), _p(g), len(g), C.byref(h)), self.h)
+        elif ranges is None:
             _check(lib().rg_batch_prepare(self.h, _p(q), len(q), _p(c), len(c), C.byref(p), C.byref(h)),
                    self.h)
         else:
@@ -371,6 +389,21 @@ class Engine:
         p = self._params(k, k1, mode)
         _check(lib().rg_search_batch_ranges(self.h, _p(q), len(q), _p(c), len(c), C.byref(p), _p(r), len(r),
                                             _p(hits), _p(counts), _p(total)), self.h)
+        return hits, counts, total
+
+    def search_batch_nested(self, queries, clauses, groups, k, k1=1.2, mode=MODE_SEARCH, ranges=None):
+        """groups (QUERY_DTYPE): the pure-SHOULD groups that CLAUSE_GROUP clauses name; ranges may be None."""
+        q = np.ascontiguousarray(queries, dtype=QUERY_DTYPE)
+        c = np.ascontiguousarray(clauses, dtype=CLAUSE_DTYPE)
+        g = np.ascontiguousarray(groups, dtype=QUERY_DTYPE)
+        r = None if ranges is None else np.ascontiguousarray(ranges, dtype=RANGE_DTYPE)
+        hits = np.zeros((len(q), k), HIT_DTYPE)
+        counts = np.zeros(len(q), np.uint32)
+        total = np.zeros(len(q), np.uint64)
+        p = self._params(k, k1, mode)
+        _check(lib().rg_search_batch_nested(self.h, _p(q), len(q), _p(c), len(c), C.byref(p), _p(r),
+                                            0 if r is None else len(r), _p(g), len(g), _p(hits), _p(counts),
+                                            _p(total)), self.h)
         return hits, counts, total
 
     def upload_points(self, seg_ord, field, bytes_per_dim, docs, packed):

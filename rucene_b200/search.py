@@ -339,6 +339,7 @@ class GpuIndexSearcher:
                         packed = np.asarray(packed, np.uint8)
                         self.engine.upload_points(ord_, fid, packed.shape[1], docs, packed)
         self._ranges = None
+        self._groups = None
         # with_similarity (searcher.rs:306-363): statistics of the largest-max_doc leaf
         # (stable sort descending -> first among equals), max_doc of the whole reader
         segs = list(reader.segments)
@@ -367,10 +368,44 @@ class GpuIndexSearcher:
         return np.float32(idf * np.float32(boost))
 
     def _compile(self, query, clauses):
-        """-> (clause_begin, n_clauses, min_should_match, flags); appends to `clauses`."""
+        """-> (clause_begin, n_clauses, min_should_match, flags); appends to `clauses`.  A group's members (see
+        _compile_one) follow the query's own clauses."""
+        pending = []
+        out = self._compile_one(query, clauses, pending)
+        for gi, members in pending:
+            begin = len(clauses)
+            for q in members.should_queries:
+                self._add_term(q, engine.SHOULD, clauses)
+            self._groups[gi] = (begin, len(members.should_queries), members.min_should_match, engine.Q_BOOLEAN)
+        return out
+
+    def _add_term(self, q, occur, clauses):
+        if not isinstance(q, TermQuery):
+            raise engine.Unsupported(engine.RG_EUNSUPPORTED, "only TermQuery leaves are accelerated")
+        if self._resolved is not None:   # ids and doc_freq came from the device dictionary
+            tid, df = self._resolved.get((q.term.field, bytes(q.term.bytes)), (None, 0))
+            doc_count = self._max_doc if self._doc_count == -1 else self._doc_count
+            w = np.float32(np.float32(codec.bm25_idf(df, doc_count)) * np.float32(q.boost))
+            clauses.append((occur, 0xFFFFFFFF if tid is None else tid, w, 0))
+            return
+        tid = self.reader.term_id(q.term)
+        absent = tid is None
+        clauses.append((occur, 0xFFFFFFFF if absent else tid, self.term_weight(None if absent else tid, q.boost), 0))
+
+    def _compile_one(self, query, clauses, pending):
         begin = len(clauses)
 
         def add(q, occur):
+            if isinstance(q, BooleanQuery) and self._groups is not None:
+                # a nested BooleanQuery: a group (RG_CLAUSE_GROUP) when it is pure SHOULD over TermQuerys; its
+                # members are written after the query's own clauses
+                if q.must_queries or q.filter_queries or q.must_not_queries or \
+                        not all(isinstance(m, TermQuery) for m in q.should_queries):
+                    raise engine.Unsupported(engine.RG_EUNSUPPORTED, "only pure-SHOULD groups of TermQuerys are accelerated")
+                clauses.append((occur | engine.CLAUSE_GROUP, len(self._groups), 0.0, 0))
+                pending.append((len(self._groups), q))
+                self._groups.append(None)
+                return
             if isinstance(q, PointRangeQuery):
                 if self._ranges is None:
                     raise engine.Unsupported(engine.RG_EUNSUPPORTED, "PointRangeQuery is not accelerated here")
@@ -383,18 +418,7 @@ class GpuIndexSearcher:
                 clauses.append((occur | engine.CLAUSE_RANGE, len(self._ranges), 0.0, 0))
                 self._ranges.append(r)
                 return
-            if not isinstance(q, TermQuery):
-                raise engine.Unsupported(engine.RG_EUNSUPPORTED, "only TermQuery leaves are accelerated")
-            if self._resolved is not None:   # ids and doc_freq came from the device dictionary
-                tid, df = self._resolved.get((q.term.field, bytes(q.term.bytes)), (None, 0))
-                doc_count = self._max_doc if self._doc_count == -1 else self._doc_count
-                w = np.float32(np.float32(codec.bm25_idf(df, doc_count)) * np.float32(q.boost))
-                clauses.append((occur, 0xFFFFFFFF if tid is None else tid, w, 0))
-                return
-            tid = self.reader.term_id(q.term)
-            absent = tid is None
-            clauses.append((occur, 0xFFFFFFFF if absent else tid,
-                            self.term_weight(None if absent else tid, q.boost), 0))
+            self._add_term(q, occur, clauses)
 
         if isinstance(query, (TermQuery, PointRangeQuery)):
             add(query, engine.SHOULD)
@@ -468,6 +492,31 @@ class GpuIndexSearcher:
         finally:
             self._ranges = None
 
+    def compile_batch_nested(self, queries):
+        """compile_batch for queries with nested pure-SHOULD BooleanQuerys (and maybe PointRangeQuerys):
+        (queries, clauses, ranges, groups) for the *_nested calls"""
+        self._ranges, self._groups = [], []
+        try:
+            q, c = self.compile_batch(queries)
+            return (q, c, np.array(self._ranges, dtype=engine.RANGE_DTYPE).reshape(-1),
+                    np.array(self._groups, dtype=engine.QUERY_DTYPE).reshape(-1))
+        finally:
+            self._ranges = self._groups = None
+
+    @staticmethod
+    def _has_groups(queries):
+        """a BooleanQuery below the top level (the lone FILTER of build() wraps its clause in a ConstantScoreQuery)"""
+        def sub(q):
+            if isinstance(q, ConstantScoreQuery):
+                return isinstance(q.query, BooleanQuery)
+            if isinstance(q, BooleanQuery):
+                return any(isinstance(s, BooleanQuery)
+                           for s in q.must_queries + q.should_queries + q.filter_queries + q.must_not_queries)
+            if isinstance(q, DisjunctionMaxQuery):
+                return any(isinstance(s, BooleanQuery) for s in q.disjuncts)
+            return False
+        return any(sub(q) for q in queries)
+
     @staticmethod
     def _has_ranges(queries):
         def walk(q):
@@ -485,18 +534,23 @@ class GpuIndexSearcher:
     def search_batch(self, queries, k, mode=engine.MODE_SEARCH, rescore=None):
         """rescore: (rescoring queries, RescoreRequest) — one rescoring query per query, the request's weights,
         mode and window for all: QueryRescorer::rescore on every row on the device before the rows are fetched."""
-        ranges = None
-        if self._has_ranges(queries):
+        ranges = groups = None
+        if self._has_groups(queries):
+            q, c, ranges, groups = self.compile_batch_nested(queries)
+        elif self._has_ranges(queries):
             q, c, ranges = self.compile_batch_ranges(queries)
         else:
             q, c = self.compile_batch(queries)
         if rescore is None:
+            if groups is not None:
+                return self.engine.search_batch_nested(q, c, groups, k, k1=self.similarity.k1, mode=mode,
+                                                       ranges=ranges)
             if ranges is not None:
                 return self.engine.search_batch_ranges(q, c, ranges, k, k1=self.similarity.k1, mode=mode)
             return self.engine.search_batch(q, c, k, k1=self.similarity.k1, mode=mode)
         rescore_queries, req = rescore
         rq, rc = self.compile_batch(rescore_queries)   # rescoring takes no ranges: a PointRangeQuery is refused
-        batch = self.engine.prepare(q, c, k, k1=self.similarity.k1, mode=mode, ranges=ranges)
+        batch = self.engine.prepare(q, c, k, k1=self.similarity.k1, mode=mode, ranges=ranges, groups=groups)
         try:
             batch.run()
             self.engine.rescore_batch(batch, rq, rc, req.window_size, req.query_weight, req.rescore_weight,
