@@ -126,7 +126,9 @@ typedef struct {
 #define RG_MODE_SEARCH_PARALLEL 1 /* search_parallel, searcher.rs:527-630: one TopDocs heap per
                                      leaf, merged in leaf order (top_docs.rs:157-172) */
 typedef struct {
-    uint32_t k;    /* TopDocsCollector::new(k), search/collector/top_docs.rs:107-113 */
+    uint32_t k;    /* TopDocsCollector::new(k), search/collector/top_docs.rs:107-113; 1..16384 (larger k is
+                      RG_EUNSUPPORTED).  For k > 1024 the kernels bound the heap root with a score histogram
+                      per work item instead of an exact running top-k: the same TopDocs, more candidates */
     float k1;      /* BM25Similarity k1, bm25_similarity.rs:45 */
     uint32_t mode; /* RG_MODE_* */
     uint32_t reserved;
@@ -325,11 +327,13 @@ typedef struct {            /* RescoreRequest, rescorer.rs:67-94 */
  * batch's).  Queued on the engine stream; rg_batch_fetch returns the rescored rows.  Calling it twice applies it
  * twice, as calling Rescorer::rescore twice would.  In RG_MODE_SEARCH_PARALLEL the rows are the merged rows
  * rg_batch_fetch returns.  Sharded runs are not covered (their hits span engines).  RG_EINVAL: the batch has not
- * run or is stale, a count mismatch, mode out of range or reserved != 0.  On any error the rows are untouched.
+ * run or is stale, a count mismatch, mode out of range or reserved != 0.  RG_EUNSUPPORTED: the batch's k is
+ * above 1024 (k_rescore sorts a row in shared memory).  On any error the rows are untouched.
  * rg_engine_last_kernel_ms(e, "rescore") times the last k_rescore launch. */
 int rg_batch_rescore(rg_engine* e, rg_batch* b, const rg_query* queries, uint32_t n_queries,
                      const rg_clause* clauses, uint32_t n_clauses, const rg_rescore_params* p);
-/* The same over caller-held TopDocs (host arrays, rows of stride k <= 1024, rewritten in place):
+/* The same over caller-held TopDocs (host arrays, rows of stride k <= 1024, rewritten in place; larger k is
+ * RG_EUNSUPPORTED):
  * Rescorer::rescore(searcher, &req, &mut top_docs) for hits that came from anywhere, e.g. the CPU searcher's answer
  * to a query the engine does not accelerate.  Synchronous.  A hit whose docid is in no leaf is RG_EINVAL. */
 int rg_rescore_hits(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
@@ -341,7 +345,8 @@ int rg_rescore_hits(rg_engine* e, const rg_query* queries, uint32_t n_queries, c
  * order == BinaryHeap::into_vec, top_docs.rs:203-213) lives on the device: */
 int rg_batch_leaf_records(rg_engine* e, rg_batch* b, void** dev_ptr, size_t* record_bytes);
 /* finish_parallel (top_docs.rs:157-172) on the device: records_all holds n_leaves consecutive
- * arrays of n_queries records (leaf order), e.g. the output of one all-gather. Host outputs. */
+ * arrays of n_queries records (leaf order), e.g. the output of one all-gather. Host outputs.  k: 1..16384, the k the
+ * records were made with (16 + 8 k bytes each). */
 int rg_merge_leaf_records(rg_engine* e, const void* dev_records_all, uint32_t n_leaves,
                           uint32_t n_queries, uint32_t k, rg_hit* out_hits, uint32_t* out_counts,
                           uint64_t* out_total_hits);

@@ -14,6 +14,8 @@ constexpr int kNoMoreDocs = 0x7fffffff;
 constexpr int kBitmapDen = 1024;      // RG_CFG_MAXSCORE: terms with df >= max_doc / 1024 get a presence bitmap at upload (within a budget)
 constexpr int kColumnDen = 64;        // terms with df >= max_doc / 64 may also get a score column (per weight, on demand)
 constexpr int kColBlk = 128;          // docids per entry of a score column's block-maximum table (ColRef::bmax)
+constexpr int kDeepBuckets = 256;     // k > 1024: score buckets of a work item's theta histogram (eval_shared.cuh)
+constexpr uint32_t kDeepMaxK = 16384; // deepest accelerated k: one replay heap of k * 8 bytes fits a CTA's shared memory
 
 // ------------------------------------------------------------------ index image in HBM
 // Every full 128-posting block pair of a term owns one 16-byte aligned slot in `arena`:

@@ -202,11 +202,13 @@ struct EvalParams {
     uint32_t* item_head;       // first run header slot per item (0xffffffff none)
     uint32_t* item_matches;    // matches per item (total_hits contribution)
     uint32_t* item_theta;      // ordered-uint running k-th best, chained item -> item+1
-    float* item_topk;          // [n_items][kcap] running top-k scores per item (see wtheta_inherit), may be null
+    float* item_topk;          // [n_items][kcap] running top-k scores per item (see wtheta_inherit), may be null;
+                               // k > kMaxK: [n_items][kDeepBuckets] u32 score histograms (see deep_inherit)
     uint32_t* item_topk_n;     // entries published per item
     uint32_t* error_flag;      // bit0: arena exhausted
     unsigned long long* dbg;   // optional event counters of k_eval_or_ms (RG_CFG_STATS), else null
     unsigned long long* touched;  // bytes k_eval_and actually asked for: decoded blocks + tables + gathers (its roofline)
+    const uint2* deep_map;     // k > kMaxK: per query the (base, shift) of its theta bucket map (eval_shared.cuh), else null
 };
 // one score column to materialise: the BM25 contributions of (leaf, term, weight, norm cache, k1);
 // a bitmap job (weight unused) sets presence bits instead

@@ -92,7 +92,8 @@ __device__ __forceinline__ uint32_t dpq_top_list(DpqWarpShared& sh, uint32_t siz
     return n;
 }
 
-template <bool LIVE>
+// DEEP: k > kMaxK — theta from a score histogram in the topk slot (kcap = kDeepBuckets, see deep_publish)
+template <bool LIVE, bool DEEP = false>
 __global__ void __launch_bounds__(kDpqWarps * 32)
 k_eval_dpq(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, uint32_t warp_bytes, uint32_t kcap) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -152,7 +153,9 @@ k_eval_dpq(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, 
     em.run_cnt = 0;
     em.matches = 0;
     em.overflow = false;
-    wtheta_inherit(em, p, item_idx, it.chain_pos, kcap, lane);
+    const uint2 dmap = DEEP ? p.deep_map[it.query] : uint2{0u, 0u};
+    if (DEEP) em.theta_local = deep_inherit(reinterpret_cast<uint32_t*>(topk), p, item_idx, it.chain_pos, dmap, lane);
+    else wtheta_inherit(em, p, item_idx, it.chain_pos, kcap, lane);
     const bool lb_ok = (uint32_t)lane < it.chain_pos;
     const uint32_t* theta_lb = p.item_theta + item_idx - 1 - (lb_ok ? lane : 0);
 
@@ -275,7 +278,8 @@ k_eval_dpq(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, 
                     if (cand) {
                         const uint32_t r = __popc(cm & ((1u << lane) - 1u));
                         p.cand_arena[em.run_slot + 1 + em.run_cnt + r] = rg_hit{h.doc + seg.doc_base, h.score};
-                        sh.newc[r] = h.score;
+                        if (DEEP) deep_count(reinterpret_cast<uint32_t*>(topk), dmap, h.score);
+                        else sh.newc[r] = h.score;
                     }
                     em.run_cnt += cn;
                     newc_n = cn;
@@ -283,7 +287,8 @@ k_eval_dpq(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, 
                 }
             }
             __syncwarp();
-            wtheta_update(em, p, item_idx, kcap, lane, sh.newc, newc_n);
+            if (DEEP) wtheta_update_deep(em, p, item_idx, dmap, lane, newc_n);
+            else wtheta_update(em, p, item_idx, kcap, lane, sh.newc, newc_n);
             __syncwarp();
             if (lane == 0) st.nout = 0;
         }
@@ -292,21 +297,24 @@ k_eval_dpq(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, 
     if (lane == 0) p.item_matches[item_idx] = matches;
 }
 
-template <bool LIVE>
+template <bool LIVE, bool DEEP = false>
 static void launch_eval_dpq_t(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n, size_t wb,
                               uint32_t kcap) {
     const size_t smem = wb * kDpqWarps;
-    cudaFuncSetAttribute(k_eval_dpq<LIVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    k_eval_dpq<LIVE><<<(n + kDpqWarps - 1) / kDpqWarps, kDpqWarps * 32, smem, st>>>(p, item_ids, n, (uint32_t)wb, kcap);
+    cudaFuncSetAttribute(k_eval_dpq<LIVE, DEEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    k_eval_dpq<LIVE, DEEP><<<(n + kDpqWarps - 1) / kDpqWarps, kDpqWarps * 32, smem, st>>>(p, item_ids, n, (uint32_t)wb, kcap);
 }
 
 void launch_eval_dpq(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n, uint32_t max_terms,
                      bool has_live) {
     if (!n) return;
-    const uint32_t kcap = (std::min<uint32_t>(p.k, kMaxK) + 31u) & ~31u;
+    const bool deep = p.k > (uint32_t)kMaxK;
+    const uint32_t kcap = deep ? (uint32_t)kDeepBuckets : (std::min<uint32_t>(p.k, kMaxK) + 31u) & ~31u;
     size_t wb = sizeof(DpqWarpShared) + (size_t)kcap * sizeof(float) + (size_t)max_terms * kBlock * 8;
     wb = (wb + 15) & ~size_t(15);
-    if (has_live) launch_eval_dpq_t<true>(st, p, item_ids, n, wb, kcap);
+    if (deep && has_live) launch_eval_dpq_t<true, true>(st, p, item_ids, n, wb, kcap);
+    else if (deep) launch_eval_dpq_t<false, true>(st, p, item_ids, n, wb, kcap);
+    else if (has_live) launch_eval_dpq_t<true>(st, p, item_ids, n, wb, kcap);
     else launch_eval_dpq_t<false>(st, p, item_ids, n, wb, kcap);
 }
 

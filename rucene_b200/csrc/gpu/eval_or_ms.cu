@@ -95,7 +95,8 @@ __device__ __forceinline__ void ms_add(uint32_t (&S)[kMsPlanes], uint32_t& over,
 }
 
 // PLANES: the batch uses tf-norm planes (RG_CFG_TFPLANES): three-level bound, two more words per clause and window
-template <bool LIVE, bool PLANES>
+// DEEP: k > kMaxK — theta from a score histogram in the topk slot (kcap = kDeepBuckets, see deep_publish)
+template <bool LIVE, bool PLANES, bool DEEP = false>
 __global__ void __launch_bounds__(kMsThreads, 24)
 k_eval_or_ms(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, uint32_t warp_bytes,
              uint32_t kcap) {
@@ -112,6 +113,7 @@ k_eval_or_ms(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids
     const SegDev seg = p.segs[it.seg];
     const int T = it.n_terms;
     const int lo = it.lo, hi = it.hi;
+    const uint2 dmap = DEEP ? p.deep_map[it.query] : uint2{0u, 0u};
 
     // ---- clauses: lane t < T owns clause t
     int kind = kKindNone;
@@ -205,7 +207,8 @@ k_eval_or_ms(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids
     em.run_cnt = 0;
     em.matches = 0;
     em.overflow = false;
-    wtheta_inherit(em, p, item_idx, it.chain_pos, kcap, lane);
+    if (DEEP) em.theta_local = deep_inherit(reinterpret_cast<uint32_t*>(topk), p, item_idx, it.chain_pos, dmap, lane);
+    else wtheta_inherit(em, p, item_idx, it.chain_pos, kcap, lane);
     const bool lb_ok = (uint32_t)lane < it.chain_pos;
     const uint32_t* theta_lb = p.item_theta + item_idx - 1 - (lb_ok ? lane : 0);
     uint32_t win_no = 0;
@@ -540,7 +543,8 @@ k_eval_or_ms(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids
                 if (cand) {
                     const uint32_t r = __popc(cm & ((1u << lane) - 1u));
                     p.cand_arena[em.run_slot + 1 + em.run_cnt + r] = rg_hit{base + idx + seg.doc_base, sc};
-                    if (newc_n + r < (uint32_t)kNewcW) sh.newc[newc_n + r] = sc;
+                    if (DEEP) deep_count(reinterpret_cast<uint32_t*>(topk), dmap, sc);
+                    else if (newc_n + r < (uint32_t)kNewcW) sh.newc[newc_n + r] = sc;
                 }
                 em.run_cnt += cn;
                 newc_n += cn;
@@ -551,7 +555,8 @@ k_eval_or_ms(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids
             // re-arm the accumulator words that were touched (E bits live in the owning lane's word)
             if ((uint32_t)lane < n_e) sh.acc[lane] = 0.0f;
             if ((uint32_t)lane + 32u < n_e) sh.acc[lane + 32] = 0.0f;
-            wtheta_update(em, p, item_idx, kcap, lane, sh.newc, newc_n);
+            if (DEEP) wtheta_update_deep(em, p, item_idx, dmap, lane, newc_n);
+            else wtheta_update(em, p, item_idx, kcap, lane, sh.newc, newc_n);
             __syncwarp();
         }
         pos = win1;
@@ -591,26 +596,33 @@ k_eval_or_ms(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids
     }
 }
 
-template <bool LIVE, bool PLANES>
+template <bool LIVE, bool PLANES, bool DEEP>
 static void launch_eval_or_ms_t(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n, size_t wb,
                                 uint32_t kcap) {
     const size_t smem = wb * kMsWarps;
     // per launch, not cached: the attribute is per device and engines may live on several
-    cudaFuncSetAttribute(k_eval_or_ms<LIVE, PLANES>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(k_eval_or_ms<LIVE, PLANES, DEEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     const uint32_t ctas = (n + kMsWarps - 1) / kMsWarps;
-    k_eval_or_ms<LIVE, PLANES><<<ctas, kMsThreads, smem, st>>>(p, item_ids, n, (uint32_t)wb, kcap);
+    k_eval_or_ms<LIVE, PLANES, DEEP><<<ctas, kMsThreads, smem, st>>>(p, item_ids, n, (uint32_t)wb, kcap);
+}
+
+template <bool DEEP>
+static void launch_eval_or_ms_d(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n,
+                                uint32_t max_streams, bool has_live, bool planes) {
+    const uint32_t kcap = DEEP ? (uint32_t)kDeepBuckets : (std::min<uint32_t>(p.k, kMaxK) + 31u) & ~31u;
+    size_t wb = sizeof(MsWarpShared) + (size_t)kcap * sizeof(float) + (size_t)max_streams * kBlock * 8;
+    wb = (wb + 15) & ~size_t(15);
+    if (has_live && planes) launch_eval_or_ms_t<true, true, DEEP>(st, p, item_ids, n, wb, kcap);
+    else if (has_live) launch_eval_or_ms_t<true, false, DEEP>(st, p, item_ids, n, wb, kcap);
+    else if (planes) launch_eval_or_ms_t<false, true, DEEP>(st, p, item_ids, n, wb, kcap);
+    else launch_eval_or_ms_t<false, false, DEEP>(st, p, item_ids, n, wb, kcap);
 }
 
 void launch_eval_or_ms(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n,
                        uint32_t max_streams, bool has_live, bool planes) {
     if (!n) return;
-    const uint32_t kcap = (std::min<uint32_t>(p.k, kMaxK) + 31u) & ~31u;
-    size_t wb = sizeof(MsWarpShared) + (size_t)kcap * sizeof(float) + (size_t)max_streams * kBlock * 8;
-    wb = (wb + 15) & ~size_t(15);
-    if (has_live && planes) launch_eval_or_ms_t<true, true>(st, p, item_ids, n, wb, kcap);
-    else if (has_live) launch_eval_or_ms_t<true, false>(st, p, item_ids, n, wb, kcap);
-    else if (planes) launch_eval_or_ms_t<false, true>(st, p, item_ids, n, wb, kcap);
-    else launch_eval_or_ms_t<false, false>(st, p, item_ids, n, wb, kcap);
+    if (p.k > (uint32_t)kMaxK) launch_eval_or_ms_d<true>(st, p, item_ids, n, max_streams, has_live, planes);
+    else launch_eval_or_ms_d<false>(st, p, item_ids, n, max_streams, has_live, planes);
 }
 
 }  // namespace rg

@@ -55,6 +55,88 @@ __device__ __forceinline__ uint32_t ld_volatile_u32(const uint32_t* p) {
     return v;
 }
 
+// ------------------------------------------------------------------------------------------
+// deep top-k (k > kMaxK): theta from a score histogram
+// ------------------------------------------------------------------------------------------
+// A batch with k > kMaxK keeps, per work item, kDeepBuckets u32 counts of its emitted candidate scores in the slot the
+// running top-k uses otherwise (WarpShared's topk, EmitShared::topk), so shared memory does not grow with k.  Per query
+// the planner picks a bucket map m = (base, shift) (EvalParams::deep_map):
+//   key(s) = clamp((float_to_ordered(s) - base) >> shift, 0, B - 1),   edge(b) = ordered_to_float(base + (b << shift))
+// for b >= 1; bucket 0 is the floor and its edge is -inf.  Since float_to_ordered is monotone, every score in bucket
+// b >= 1 is >= edge(b), whatever range the map was sized for (a score above it clamps into bucket B - 1).
+//
+// theta = edge(b) for the largest b whose suffix count (buckets b..B-1) is >= k.  Why that is exact: the counts are of
+// candidates this item (and, through deep_inherit, the earlier items of its heap chain) already emitted, each doc at
+// most once along the chain, all of them earlier in collection order.  So at least k earlier-collected docs score
+// >= edge(b), the heap root is >= edge(b) once the replay gets here, and a doc with score <= edge(b) cannot replace it
+// (TopDocsCollector replaces the root only when root.score < score, top_docs.rs:67-76).  Counts only grow: a copy that
+// races with a predecessor's increments undercounts and the bound stays valid, so the histogram needs no
+// count-then-entries protocol, only volatile reads.  A NaN score is never counted.
+__device__ __forceinline__ uint32_t deep_key(uint2 m, float s) {
+    const uint32_t o = float_to_ordered(s);
+    return o < m.x ? 0u : min((o - m.x) >> m.y, (uint32_t)(kDeepBuckets - 1));
+}
+
+__device__ __forceinline__ void deep_count(uint32_t* hist, uint2 m, float s) {
+    if (s == s) atomicAdd(hist + deep_key(m, s), 1u);
+}
+
+// Warp-cooperative (lane l owns buckets [8l, 8l + 8)): theta of the histogram; mirrors it into
+// EvalParams::item_topk[item] (stride kDeepBuckets), then publishes its total in item_topk_n[item] and theta in
+// item_theta[item].
+__device__ __forceinline__ float deep_publish(const uint32_t* hist, const EvalParams& p, uint32_t item_idx, uint2 m, int lane) {
+    uint32_t* g = p.item_topk ? reinterpret_cast<uint32_t*>(p.item_topk) + (size_t)item_idx * kDeepBuckets : nullptr;
+    uint32_t c[8], own = 0;
+#pragma unroll
+    for (int j = 0; j < 8; j++) {
+        c[j] = hist[lane * 8 + j];
+        own += c[j];
+        if (g) g[lane * 8 + j] = c[j];
+    }
+    uint32_t suf = own;  // buckets of lanes >= this one
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+        const uint32_t v = __shfl_down_sync(0xffffffffu, suf, o);
+        if (lane + o < 32) suf += v;
+    }
+    const uint32_t total = __shfl_sync(0xffffffffu, suf, 0);
+    int best = -1;
+    uint32_t s = suf - own;
+#pragma unroll
+    for (int j = 7; j >= 0; j--) {
+        s += c[j];
+        if (best < 0 && s >= p.k) best = lane * 8 + j;
+    }
+    best = __reduce_max_sync(0xffffffffu, best);
+    const float theta = best >= 1 ? ordered_to_float(m.x + ((uint32_t)best << m.y)) : -INFINITY;
+    if (lane == 0) {
+        if (g && total) {  // buckets first, then the total a successor looks for
+            __threadfence();
+            *reinterpret_cast<volatile uint32_t*>(p.item_topk_n + item_idx) = total;
+        }
+        if (theta != -INFINITY) atomicMax(p.item_theta + item_idx, float_to_ordered(theta));
+    }
+    return theta;
+}
+
+// Warp-cooperative start of a deep work item: copy the nearest predecessor's published histogram into `hist` (zeros
+// when there is none) and return its theta.
+__device__ __forceinline__ float deep_inherit(uint32_t* hist, const EvalParams& p, uint32_t item_idx, uint32_t chain_pos,
+                                           uint2 m, int lane) {
+    const uint32_t* src = nullptr;
+    if (p.item_topk && chain_pos) {
+        const uint32_t cnt = (uint32_t)lane < chain_pos ? ld_volatile_u32(p.item_topk_n + item_idx - 1 - lane) : 0u;
+        const uint32_t have = __ballot_sync(0xffffffffu, cnt > 0u);
+        if (have) src = reinterpret_cast<const uint32_t*>(p.item_topk) + (size_t)(item_idx - (uint32_t)__ffs(have)) * kDeepBuckets;
+        __threadfence();
+    }
+#pragma unroll
+    for (int j = 0; j < 8; j++) hist[lane * 8 + j] = src ? ld_volatile_u32(src + lane * 8 + j) : 0u;
+    __syncwarp();
+    if (!src) return -INFINITY;
+    return deep_publish(hist, p, item_idx, m, lane);
+}
+
 // warp 0: fold this window's candidate scores into the running top-k and publish theta
 static __device__ void theta_update(EmitShared& es, uint32_t k, uint32_t* theta_out) {
     const int lane = lane_id();
@@ -109,12 +191,27 @@ static __device__ void theta_update(EmitShared& es, uint32_t k, uint32_t* theta_
     }
 }
 
+// warp 0, deep batches: theta from the histogram in es.topk (when the window emitted something); publish theta
+static __device__ void theta_update_deep(EmitShared& es, const EvalParams& p, uint32_t item_idx, uint2 m) {
+    const int lane = lane_id();
+    if (es.newc_n) {
+        const float theta = deep_publish(reinterpret_cast<const uint32_t*>(es.topk), p, item_idx, m, lane);
+        if (lane == 0) es.theta_local = theta;
+    }
+    if (lane == 0) {
+        uint32_t ord = es.theta_in;
+        if (es.theta_local != -INFINITY) ord = max(ord, float_to_ordered(es.theta_local));
+        if (ord > kOrderedNegInf) atomicMax(p.item_theta + item_idx, ord);
+    }
+}
+
 // One emission step.  Slot order = (warp, step, lane) ascending == docid order.  `present`
 // marks matches; inherited_theta is thread 0's prefetched copy of the previous item's theta.
-template <int STEPS>
+// DEEP (k > kMaxK): candidates are counted in the histogram of the query's bucket map `dmap` instead.
+template <int STEPS, bool DEEP = false>
 __device__ void emit_window(EmitShared& es, const EvalParams& p, uint32_t item_idx, int doc_base,
                             const bool (&present)[STEPS], const int (&doc)[STEPS],
-                            const float (&score)[STEPS], uint32_t inherited_theta) {
+                            const float (&score)[STEPS], uint32_t inherited_theta, uint2 dmap = uint2{0u, 0u}) {
     const int lane = lane_id(), warp = threadIdx.x >> 5;
     float te = es.theta_local;
     if (es.theta_in > kOrderedNegInf) te = fmaxf(te, ordered_to_float(es.theta_in));
@@ -177,13 +274,17 @@ __device__ void emit_window(EmitShared& es, const EvalParams& p, uint32_t item_i
             if ((cmask[s] >> lane) & 1u) {
                 p.cand_arena[pos + __popc(cmask[s] & lt)] = rg_hit{doc[s] + doc_base, score[s]};
                 const uint32_t i = atomicAdd(&es.newc_n, 1u);
-                if (i < (uint32_t)kNewcMax) es.newc[i] = score[s];
+                if (DEEP) deep_count(reinterpret_cast<uint32_t*>(es.topk), dmap, score[s]);
+                else if (i < (uint32_t)kNewcMax) es.newc[i] = score[s];
             }
             pos += __popc(cmask[s]);
         }
     }
     __syncthreads();
-    if (warp == 0) theta_update(es, p.k, p.item_theta + item_idx);
+    if (warp == 0) {
+        if (DEEP) theta_update_deep(es, p, item_idx, dmap);
+        else theta_update(es, p.k, p.item_theta + item_idx);
+    }
 }
 
 // first index in [lo, hi) with a[i] >= key (hi if none)
@@ -454,6 +555,14 @@ __device__ __forceinline__ void wtheta_inherit(WEmit& em, const EvalParams& p, u
         *reinterpret_cast<volatile uint32_t*>(p.item_topk_n + item_idx) = n;
         if (em.theta_local != -INFINITY) atomicMax(p.item_theta + item_idx, float_to_ordered(em.theta_local));
     }
+}
+
+// the warp kernels' update after a window: only when it emitted something
+__device__ __forceinline__ void wtheta_update_deep(WEmit& em, const EvalParams& p, uint32_t item_idx, uint2 m, int lane,
+                                                   uint32_t emitted) {
+    if (emitted == 0) return;
+    __syncwarp();
+    em.theta_local = deep_publish(reinterpret_cast<const uint32_t*>(em.topk), p, item_idx, m, lane);
 }
 
 // Refill clause t's stream cache with its next block (or vint tail): unpack, docid scan, norm

@@ -252,7 +252,8 @@ __device__ __forceinline__ int list_window(uint32_t* acc, WTerm& tc, int win0, i
 
 // LEAN: the decode-free variant for plain-sum items (POS) whose every clause is a score column or a scored list —
 // no block decode, no stream cache in shared memory, so fewer registers and more resident warps.
-template <bool LIVE, bool NOT, bool MSM, bool DMAX, bool POS, bool LEAN = false>
+// DEEP: k > kMaxK — theta from a score histogram in the topk slot (kcap = kDeepBuckets, see deep_publish).
+template <bool LIVE, bool NOT, bool MSM, bool DMAX, bool POS, bool LEAN = false, bool DEEP = false>
 __global__ void __launch_bounds__(kOrThreads, LEAN ? 32 : 24)
 k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, uint32_t warp_bytes,
           uint32_t kcap) {
@@ -271,6 +272,7 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
     const int T = it.n_terms;
     const int lo = it.lo, hi = it.hi;
     float* cscores = reinterpret_cast<float*>(cdocs + T * kBlock);
+    const uint2 dmap = DEEP ? p.deep_map[it.query] : uint2{0u, 0u};
 
     for (int i = lane; i < kWw; i += 32) sh.acc[i] = POS ? 0u : kSent;
     MsmCtx mc;
@@ -356,7 +358,8 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
     em.run_cnt = 0;
     em.matches = 0;
     em.overflow = false;
-    wtheta_inherit(em, p, item_idx, it.chain_pos, kcap, lane);
+    if (DEEP) em.theta_local = deep_inherit(reinterpret_cast<uint32_t*>(topk), p, item_idx, it.chain_pos, dmap, lane);
+    else wtheta_inherit(em, p, item_idx, it.chain_pos, kcap, lane);
     // theta look-back: the up-to-32 preceding items of this heap chain (each publishes
     // max(own, inherited)), re-read every 8 windows
     const bool lb_ok = (uint32_t)lane < it.chain_pos;
@@ -531,7 +534,8 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
                 if (cand) {
                     const uint32_t r = __popc(cm & ((1u << lane) - 1u));
                     p.cand_arena[em.run_slot + 1 + em.run_cnt + r] = rg_hit{win0 + idx + seg.doc_base, sc};
-                    if (newc_n + r < (uint32_t)kNewcW) sh.newc[newc_n + r] = sc;
+                    if (DEEP) deep_count(reinterpret_cast<uint32_t*>(topk), dmap, sc);
+                    else if (newc_n + r < (uint32_t)kNewcW) sh.newc[newc_n + r] = sc;
                 }
                 em.run_cnt += c;
                 newc_n += c;
@@ -546,7 +550,8 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
             if (MSM) {
                 for (int i = lane; i < kWw / 16; i += 32) reinterpret_cast<uint4*>(mc.cnt)[i] = make_uint4(0, 0, 0, 0);
             }
-            wtheta_update(em, p, item_idx, kcap, lane, sh.newc, newc_n);
+            if (DEEP) wtheta_update_deep(em, p, item_idx, dmap, lane, newc_n);
+            else wtheta_update(em, p, item_idx, kcap, lane, sh.newc, newc_n);
             __syncwarp();
         }
         if (next_doc == kNoMoreDocs) break;
@@ -631,7 +636,8 @@ __device__ __forceinline__ bool range_hit(const RangeRef& r, int d) {
 // block per warp.  Without it the body is the plain conjunction / ReqOpt kernel, unchanged.
 // GROUPS: the item has pure-SHOULD groups of terms (ItemClause bits 9-11, see AndSharedN); a group that leads merges
 // its members' postings in docid order.  gstats: group-lead counters (GROUPS only).
-template <bool REQOPT, bool OTHER, bool RANGES, bool GROUPS = false>
+// DEEP: k > kMaxK — theta from a score histogram in EmitShared::topk (see deep_publish).
+template <bool REQOPT, bool OTHER, bool RANGES, bool GROUPS = false, bool DEEP = false>
 __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_t* __restrict__ item_ids,
                                               const RangeParams& rp, unsigned long long* gstats = nullptr) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -675,6 +681,11 @@ __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_
     }
     const uint32_t* theta_prev = (it.chain_pos == 0) ? nullptr : p.item_theta + (item_idx - 1);
     if (RANGES && threadIdx.x == 0) shr.rcur = (uint32_t)lo / kBlock;
+    const uint2 dmap = DEEP ? p.deep_map[it.query] : uint2{0u, 0u};
+    if (DEEP && warp == 0) {
+        const float th = deep_inherit(reinterpret_cast<uint32_t*>(sh.emit.topk), p, item_idx, it.chain_pos, dmap, lane);
+        if (lane == 0) sh.emit.theta_local = th;
+    }
     __syncthreads();
 
     const TermCtx& lead = sh.term[0];
@@ -1184,7 +1195,7 @@ __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_
             score[s] = sh.lscore[slot];
             present[s] = doc[s] != kNoMoreDocs && is_live(seg, doc[s]);
         }
-        emit_window<kAndSteps>(sh.emit, p, item_idx, seg.doc_base, present, doc, score, inherited);
+        emit_window<kAndSteps, DEEP>(sh.emit, p, item_idx, seg.doc_base, present, doc, score, inherited, dmap);
         __syncthreads();
     }
     __syncthreads();
@@ -1203,22 +1214,22 @@ __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_
     }
 }
 
-template <bool REQOPT, bool OTHER>
+template <bool REQOPT, bool OTHER, bool DEEP = false>
 __global__ void __launch_bounds__(kEvalThreads, OTHER ? (REQOPT ? 4 : 5) : 0)  // the decoder call must not cost occupancy
 k_eval_and(EvalParams p, const uint32_t* __restrict__ item_ids) {
-    eval_and_body<REQOPT, OTHER, false>(p, item_ids, RangeParams{});
+    eval_and_body<REQOPT, OTHER, false, false, DEEP>(p, item_ids, RangeParams{});
 }
 
-template <bool REQOPT, bool OTHER>
+template <bool REQOPT, bool OTHER, bool DEEP = false>
 __global__ void __launch_bounds__(kEvalThreads, OTHER ? (REQOPT ? 4 : 5) : 0)
 k_eval_and_ranges(EvalParams p, const uint32_t* __restrict__ item_ids, RangeParams rp) {
-    eval_and_body<REQOPT, OTHER, true>(p, item_ids, rp);
+    eval_and_body<REQOPT, OTHER, true, false, DEEP>(p, item_ids, rp);
 }
 
-template <bool REQOPT, bool OTHER>
+template <bool REQOPT, bool OTHER, bool DEEP = false>
 __global__ void __launch_bounds__(kEvalThreads, OTHER ? (REQOPT ? 4 : 5) : 0)
 k_eval_and_nested(EvalParams p, const uint32_t* __restrict__ item_ids, RangeParams rp, unsigned long long* gstats) {
-    eval_and_body<REQOPT, OTHER, true, true>(p, item_ids, rp, gstats);
+    eval_and_body<REQOPT, OTHER, true, true, DEEP>(p, item_ids, rp, gstats);
 }
 
 // ------------------------------------------------------------------------------------------
@@ -1331,11 +1342,13 @@ __device__ void finish_sorted(Heap& hp, unsigned long long total, rg_hit* out, u
     }
 }
 
-__global__ void __launch_bounds__(kReplayWarps * 32)
+// WARPS heaps per CTA: kReplayWarps for k <= kMaxK; one for deeper heaps (k * 8 bytes of shared memory each)
+template <int WARPS>
+__global__ void __launch_bounds__(WARPS * 32)
 k_heap_replay(ReplayParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5, lane = lane_id();
-    const uint32_t g = blockIdx.x * kReplayWarps + warp;
+    const uint32_t g = blockIdx.x * WARPS + warp;
     if (g >= p.n_groups) return;
     Heap hp;
     hp.data = reinterpret_cast<rg_hit*>(smem_raw) + (size_t)warp * p.k;
@@ -1370,13 +1383,14 @@ k_heap_replay(ReplayParams p) {
 }
 
 // finish_parallel (top_docs.rs:157-172): leaves in leaf order, each leaf's docs in heap-array
-// order through add_doc; total_hits summed.
-__global__ void __launch_bounds__(kReplayWarps * 32)
+// order through add_doc; total_hits summed.  WARPS as for k_heap_replay.
+template <int WARPS>
+__global__ void __launch_bounds__(WARPS * 32)
 k_merge_leaf_records(const uint8_t* __restrict__ records, uint32_t n_leaves, uint32_t n_queries,
                      uint32_t k, rg_hit* out_hits, uint32_t* out_counts, unsigned long long* out_total) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const int warp = threadIdx.x >> 5;
-    const uint32_t q = blockIdx.x * kReplayWarps + warp;
+    const uint32_t q = blockIdx.x * WARPS + warp;
     if (q >= n_queries) return;
     Heap hp;
     hp.data = reinterpret_cast<rg_hit*>(smem_raw) + (size_t)warp * k;
@@ -1548,106 +1562,148 @@ void launch_build_tf_planes(cudaStream_t st, const SegDev* segs, const ColumnJob
     if (hist) k_build_columns<3><<<ctas, kColWarps * 32, 0, st>>>(segs, jobs, n_jobs, n_units, caches, k1, hist, 0);
     else k_build_columns<2><<<ctas, kColWarps * 32, 0, st>>>(segs, jobs, n_jobs, n_units, caches, k1, nullptr, plane_stride);
 }
-template <bool LIVE, bool NOT, bool MSM, bool DMAX, bool POS = false, bool LEAN = false>
+template <bool LIVE, bool NOT, bool MSM, bool DMAX, bool POS = false, bool LEAN = false, bool DEEP = false>
 static void launch_eval_or_t(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n, size_t wb,
                              uint32_t kcap) {
     const size_t smem = wb * kOrWarps;
     // per launch, not cached: the attribute is per device and engines may live on several
-    cudaFuncSetAttribute(k_eval_or<LIVE, NOT, MSM, DMAX, POS, LEAN>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaFuncSetAttribute(k_eval_or<LIVE, NOT, MSM, DMAX, POS, LEAN, DEEP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     const uint32_t ctas = (n + kOrWarps - 1) / kOrWarps;
-    k_eval_or<LIVE, NOT, MSM, DMAX, POS, LEAN><<<ctas, kOrThreads, smem, st>>>(p, item_ids, n, (uint32_t)wb, kcap);
+    k_eval_or<LIVE, NOT, MSM, DMAX, POS, LEAN, DEEP><<<ctas, kOrThreads, smem, st>>>(p, item_ids, n, (uint32_t)wb, kcap);
 }
 // plain-sum items whose every clause is a score column or a scored list (no stream cache in shared memory)
 void launch_eval_or_lean(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n, bool has_live) {
     if (!n) return;
-    const uint32_t kcap = (std::min<uint32_t>(p.k, kMaxK) + 31u) & ~31u;
+    const bool deep = p.k > (uint32_t)kMaxK;
+    const uint32_t kcap = deep ? (uint32_t)kDeepBuckets : (std::min<uint32_t>(p.k, kMaxK) + 31u) & ~31u;
     const size_t wb = (sizeof(WarpShared) + (size_t)kcap * sizeof(float) + 15) & ~size_t(15);
-    if (has_live) launch_eval_or_t<true, false, false, false, true, true>(st, p, item_ids, n, wb, kcap);
+    if (deep && has_live) launch_eval_or_t<true, false, false, false, true, true, true>(st, p, item_ids, n, wb, kcap);
+    else if (deep) launch_eval_or_t<false, false, false, false, true, true, true>(st, p, item_ids, n, wb, kcap);
+    else if (has_live) launch_eval_or_t<true, false, false, false, true, true>(st, p, item_ids, n, wb, kcap);
     else launch_eval_or_t<false, false, false, false, true, true>(st, p, item_ids, n, wb, kcap);
 }
+template <bool DEEP>
+static void launch_eval_or_d(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n,
+                             uint32_t max_terms, bool has_live, bool has_not, bool has_msm, bool has_dmax, bool all_pos);
 // has_live: some leaf has deleted docs; has_not: some item of the launch carries a MUST_NOT clause;
 // all_pos: every clause score of every item of the launch is > 0 (the planner checked weights and norm caches)
 void launch_eval_or(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n,
                     uint32_t max_terms, bool has_live, bool has_not, bool has_msm, bool has_dmax, bool all_pos) {
     if (!n) return;
-    const uint32_t kcap = (std::min<uint32_t>(p.k, kMaxK) + 31u) & ~31u;
+    if (p.k > (uint32_t)kMaxK) launch_eval_or_d<true>(st, p, item_ids, n, max_terms, has_live, has_not, has_msm, has_dmax, all_pos);
+    else launch_eval_or_d<false>(st, p, item_ids, n, max_terms, has_live, has_not, has_msm, has_dmax, all_pos);
+}
+template <bool DEEP>
+static void launch_eval_or_d(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n,
+                             uint32_t max_terms, bool has_live, bool has_not, bool has_msm, bool has_dmax, bool all_pos) {
+    const uint32_t kcap = DEEP ? (uint32_t)kDeepBuckets : (std::min<uint32_t>(p.k, kMaxK) + 31u) & ~31u;
     size_t wb = sizeof(WarpShared) + (size_t)kcap * sizeof(float) + (size_t)max_terms * kBlock * 8;
     wb = (wb + 15) & ~size_t(15);
     if (has_dmax) {  // a DisjunctionMaxQuery in the batch: per-doc counters + per-doc maxima
         wb += kWw + kWw * sizeof(float);
         wb = (wb + 15) & ~size_t(15);
-        launch_eval_or_t<true, true, true, true>(st, p, item_ids, n, wb, kcap);
+        launch_eval_or_t<true, true, true, true, false, false, DEEP>(st, p, item_ids, n, wb, kcap);
     } else if (has_msm) {  // min_should_match > 1 somewhere in the batch: the general sum variant
         wb += kWw;  // per-doc clause counters
         wb = (wb + 15) & ~size_t(15);
-        launch_eval_or_t<true, true, true, false>(st, p, item_ids, n, wb, kcap);
-    } else if (has_live && has_not) launch_eval_or_t<true, true, false, false>(st, p, item_ids, n, wb, kcap);
-    else if (has_not) launch_eval_or_t<false, true, false, false>(st, p, item_ids, n, wb, kcap);
-    else if (has_live && all_pos) launch_eval_or_t<true, false, false, false, true>(st, p, item_ids, n, wb, kcap);
-    else if (all_pos) launch_eval_or_t<false, false, false, false, true>(st, p, item_ids, n, wb, kcap);
-    else if (has_live) launch_eval_or_t<true, false, false, false>(st, p, item_ids, n, wb, kcap);
-    else launch_eval_or_t<false, false, false, false>(st, p, item_ids, n, wb, kcap);
+        launch_eval_or_t<true, true, true, false, false, false, DEEP>(st, p, item_ids, n, wb, kcap);
+    } else if (has_live && has_not) launch_eval_or_t<true, true, false, false, false, false, DEEP>(st, p, item_ids, n, wb, kcap);
+    else if (has_not) launch_eval_or_t<false, true, false, false, false, false, DEEP>(st, p, item_ids, n, wb, kcap);
+    else if (has_live && all_pos) launch_eval_or_t<true, false, false, false, true, false, DEEP>(st, p, item_ids, n, wb, kcap);
+    else if (all_pos) launch_eval_or_t<false, false, false, false, true, false, DEEP>(st, p, item_ids, n, wb, kcap);
+    else if (has_live) launch_eval_or_t<true, false, false, false, false, false, DEEP>(st, p, item_ids, n, wb, kcap);
+    else launch_eval_or_t<false, false, false, false, false, false, DEEP>(st, p, item_ids, n, wb, kcap);
 }
-template <bool REQOPT, bool OTHER>
+template <bool REQOPT, bool OTHER, bool DEEP>
 static void launch_eval_and_t(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n) {
-    cudaFuncSetAttribute(k_eval_and<REQOPT, OTHER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaFuncSetAttribute(k_eval_and<REQOPT, OTHER, DEEP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                          (int)sizeof(AndShared));
-    k_eval_and<REQOPT, OTHER><<<n, kEvalThreads, sizeof(AndShared), st>>>(p, item_ids);
+    k_eval_and<REQOPT, OTHER, DEEP><<<n, kEvalThreads, sizeof(AndShared), st>>>(p, item_ids);
+}
+template <bool DEEP>
+static void launch_eval_and_d(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n, bool req_opt,
+                              bool has_other_enc) {
+    if (req_opt && has_other_enc) launch_eval_and_t<true, true, DEEP>(st, p, item_ids, n);
+    else if (req_opt) launch_eval_and_t<true, false, DEEP>(st, p, item_ids, n);
+    else if (has_other_enc) launch_eval_and_t<false, true, DEEP>(st, p, item_ids, n);
+    else launch_eval_and_t<false, false, DEEP>(st, p, item_ids, n);
 }
 void launch_eval_and(cudaStream_t st, const EvalParams& p, const uint32_t* item_ids, uint32_t n, bool req_opt,
                      bool has_other_enc) {
     if (!n) return;
-    if (req_opt && has_other_enc) launch_eval_and_t<true, true>(st, p, item_ids, n);
-    else if (req_opt) launch_eval_and_t<true, false>(st, p, item_ids, n);
-    else if (has_other_enc) launch_eval_and_t<false, true>(st, p, item_ids, n);
-    else launch_eval_and_t<false, false>(st, p, item_ids, n);
+    if (p.k > (uint32_t)kMaxK) launch_eval_and_d<true>(st, p, item_ids, n, req_opt, has_other_enc);
+    else launch_eval_and_d<false>(st, p, item_ids, n, req_opt, has_other_enc);
 }
-template <bool REQOPT, bool OTHER>
+template <bool REQOPT, bool OTHER, bool DEEP>
 static void launch_eval_and_ranges_t(cudaStream_t st, const EvalParams& p, const RangeParams& rp,
                                      const uint32_t* item_ids, uint32_t n) {
-    cudaFuncSetAttribute(k_eval_and_ranges<REQOPT, OTHER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaFuncSetAttribute(k_eval_and_ranges<REQOPT, OTHER, DEEP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                          (int)sizeof(AndSharedR));
-    k_eval_and_ranges<REQOPT, OTHER><<<n, kEvalThreads, sizeof(AndSharedR), st>>>(p, item_ids, rp);
+    k_eval_and_ranges<REQOPT, OTHER, DEEP><<<n, kEvalThreads, sizeof(AndSharedR), st>>>(p, item_ids, rp);
+}
+template <bool DEEP>
+static void launch_eval_and_ranges_d(cudaStream_t st, const EvalParams& p, const RangeParams& rp,
+                                     const uint32_t* item_ids, uint32_t n, bool req_opt, bool has_other_enc) {
+    if (req_opt && has_other_enc) launch_eval_and_ranges_t<true, true, DEEP>(st, p, rp, item_ids, n);
+    else if (req_opt) launch_eval_and_ranges_t<true, false, DEEP>(st, p, rp, item_ids, n);
+    else if (has_other_enc) launch_eval_and_ranges_t<false, true, DEEP>(st, p, rp, item_ids, n);
+    else launch_eval_and_ranges_t<false, false, DEEP>(st, p, rp, item_ids, n);
 }
 void launch_eval_and_ranges(cudaStream_t st, const EvalParams& p, const RangeParams& rp, const uint32_t* item_ids,
                             uint32_t n, bool req_opt, bool has_other_enc) {
     if (!n) return;
-    if (req_opt && has_other_enc) launch_eval_and_ranges_t<true, true>(st, p, rp, item_ids, n);
-    else if (req_opt) launch_eval_and_ranges_t<true, false>(st, p, rp, item_ids, n);
-    else if (has_other_enc) launch_eval_and_ranges_t<false, true>(st, p, rp, item_ids, n);
-    else launch_eval_and_ranges_t<false, false>(st, p, rp, item_ids, n);
+    if (p.k > (uint32_t)kMaxK) launch_eval_and_ranges_d<true>(st, p, rp, item_ids, n, req_opt, has_other_enc);
+    else launch_eval_and_ranges_d<false>(st, p, rp, item_ids, n, req_opt, has_other_enc);
 }
-template <bool REQOPT, bool OTHER>
+template <bool REQOPT, bool OTHER, bool DEEP>
 static void launch_eval_and_nested_t(cudaStream_t st, const EvalParams& p, const RangeParams& rp,
                                      unsigned long long* gstats, const uint32_t* item_ids, uint32_t n) {
-    cudaFuncSetAttribute(k_eval_and_nested<REQOPT, OTHER>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+    cudaFuncSetAttribute(k_eval_and_nested<REQOPT, OTHER, DEEP>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                          (int)sizeof(AndSharedN));
-    k_eval_and_nested<REQOPT, OTHER><<<n, kEvalThreads, sizeof(AndSharedN), st>>>(p, item_ids, rp, gstats);
+    k_eval_and_nested<REQOPT, OTHER, DEEP><<<n, kEvalThreads, sizeof(AndSharedN), st>>>(p, item_ids, rp, gstats);
+}
+template <bool DEEP>
+static void launch_eval_and_nested_d(cudaStream_t st, const EvalParams& p, const RangeParams& rp,
+                                     unsigned long long* gstats, const uint32_t* item_ids, uint32_t n, bool req_opt,
+                                     bool has_other_enc) {
+    if (req_opt && has_other_enc) launch_eval_and_nested_t<true, true, DEEP>(st, p, rp, gstats, item_ids, n);
+    else if (req_opt) launch_eval_and_nested_t<true, false, DEEP>(st, p, rp, gstats, item_ids, n);
+    else if (has_other_enc) launch_eval_and_nested_t<false, true, DEEP>(st, p, rp, gstats, item_ids, n);
+    else launch_eval_and_nested_t<false, false, DEEP>(st, p, rp, gstats, item_ids, n);
 }
 void launch_eval_and_nested(cudaStream_t st, const EvalParams& p, const RangeParams& rp, unsigned long long* gstats,
                             const uint32_t* item_ids, uint32_t n, bool req_opt, bool has_other_enc) {
     if (!n) return;
-    if (req_opt && has_other_enc) launch_eval_and_nested_t<true, true>(st, p, rp, gstats, item_ids, n);
-    else if (req_opt) launch_eval_and_nested_t<true, false>(st, p, rp, gstats, item_ids, n);
-    else if (has_other_enc) launch_eval_and_nested_t<false, true>(st, p, rp, gstats, item_ids, n);
-    else launch_eval_and_nested_t<false, false>(st, p, rp, gstats, item_ids, n);
+    if (p.k > (uint32_t)kMaxK) launch_eval_and_nested_d<true>(st, p, rp, gstats, item_ids, n, req_opt, has_other_enc);
+    else launch_eval_and_nested_d<false>(st, p, rp, gstats, item_ids, n, req_opt, has_other_enc);
+}
+template <int WARPS>
+static void launch_heap_replay_t(cudaStream_t st, const ReplayParams& p) {
+    const size_t smem = (size_t)WARPS * p.k * sizeof(rg_hit);
+    // per launch, not cached: the attribute is per device and engines may live on several
+    cudaFuncSetAttribute(k_heap_replay<WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    k_heap_replay<WARPS><<<(p.n_groups + WARPS - 1) / WARPS, WARPS * 32, smem, st>>>(p);
 }
 void launch_heap_replay(cudaStream_t st, const ReplayParams& p) {
     if (!p.n_groups) return;
-    const size_t smem = (size_t)kReplayWarps * p.k * sizeof(rg_hit);
+    if (p.k > (uint32_t)kMaxK) launch_heap_replay_t<1>(st, p);
+    else launch_heap_replay_t<kReplayWarps>(st, p);
+}
+template <int WARPS>
+static void launch_merge_leaf_records_t(cudaStream_t st, const uint8_t* records, uint32_t n_leaves, uint32_t n_queries,
+                                        uint32_t k, rg_hit* out_hits, uint32_t* out_counts, unsigned long long* out_total) {
+    const size_t smem = (size_t)WARPS * k * sizeof(rg_hit);
     // per launch, not cached: the attribute is per device and engines may live on several
-    cudaFuncSetAttribute(k_heap_replay, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    k_heap_replay<<<(p.n_groups + kReplayWarps - 1) / kReplayWarps, kReplayWarps * 32, smem, st>>>(p);
+    cudaFuncSetAttribute(k_merge_leaf_records<WARPS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    k_merge_leaf_records<WARPS><<<(n_queries + WARPS - 1) / WARPS, WARPS * 32, smem, st>>>(
+        records, n_leaves, n_queries, k, out_hits, out_counts, out_total);
 }
 void launch_merge_leaf_records(cudaStream_t st, const uint8_t* records, uint32_t n_leaves,
                                uint32_t n_queries, uint32_t k, rg_hit* out_hits,
                                uint32_t* out_counts, unsigned long long* out_total) {
     if (!n_queries) return;
-    const size_t smem = (size_t)kReplayWarps * k * sizeof(rg_hit);
-    // per launch, not cached: the attribute is per device and engines may live on several
-    cudaFuncSetAttribute(k_merge_leaf_records, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-    k_merge_leaf_records<<<(n_queries + kReplayWarps - 1) / kReplayWarps, kReplayWarps * 32, smem, st>>>(
-        records, n_leaves, n_queries, k, out_hits, out_counts, out_total);
+    if (k > (uint32_t)kMaxK) launch_merge_leaf_records_t<1>(st, records, n_leaves, n_queries, k, out_hits, out_counts, out_total);
+    else launch_merge_leaf_records_t<kReplayWarps>(st, records, n_leaves, n_queries, k, out_hits, out_counts, out_total);
 }
 
 }  // namespace rg

@@ -64,6 +64,7 @@ struct rg_batch {
     Span<uint32_t> item_head, item_matches, item_theta, item_topk_n;
     Span<float> item_topk;  // [n_items][kcap] (not zeroed: item_topk_n says what is valid)
     uint32_t topk_cap = 0;
+    Span<uint2> deep_map;   // k > 1024 only: per query the (base, shift) of its theta bucket map (deep_bucket_maps)
     Span<unsigned long long> arena_next;  // [0] bump pointer, [1] error flag (as u32 view)
     Span<unsigned long long> dbg;         // RG_CFG_STATS counters (zeroed per run)
     Span<rg_hit> out_hits;
@@ -1830,6 +1831,45 @@ void ensure_arena(rg_engine* e) {
     e->cand_arena.alloc(want / sizeof(rg_hit));
 }
 
+// k > 1024: the (base, shift) of every query's theta bucket map (eval_shared.cuh: deep_key).  The map only sets the
+// resolution of theta, never its validity.  With a finite positive bound U on the query's scores, the top bucket starts
+// at U and the 255 below it are 1/32 octave wide (shift 18: 2^18 ordered steps, a float octave being 2^23), covering
+// 8 octaves; else (negative or zero weights, norm caches with negative entries) the absolute map base 0, shift 24.
+// U is the largest over the query's work items of the round-up sum of its scoring clauses' nextafter(weight*(k1+1))
+// (BM25's tf-norm factor is < 1 for norms >= 0); ranges, MUST_NOT, match-all and zero-weight clauses add nothing, a
+// group's members each add their own.
+static std::vector<uint2> deep_bucket_maps(const rg_engine* e, const HostPlan& hp, uint32_t n_queries, float k1) {
+    std::vector<float> ub(n_queries, 0.0f);
+    for (const WorkItem& it : hp.items) {
+        float u = 0.0f;
+        for (uint32_t c = 0; c < it.n_terms; c++) {
+            const ItemClause& ic = hp.clauses[it.clause_begin + c];
+            if (ic.flags & (1u | 8u | 64u | 256u)) continue;
+            const float w1 = ic.weight * (k1 + 1.0f);
+            if (w1 == 0.0f) continue;  // scores +-0 only (FILTER): an all-zero query keeps the absolute map, whose edge 128 is +0
+            const bool nonneg = ic.cache_id < e->cache_nonneg.size() && e->cache_nonneg[ic.cache_id];
+            if (!(w1 >= 0.0f) || !(w1 < INFINITY) || !(k1 >= 0.0f) || !nonneg) {
+                u = INFINITY;
+                break;
+            }
+            u = nextafterf(u + nextafterf(w1, INFINITY), INFINITY);
+        }
+        ub[it.query] = std::max(ub[it.query], u);
+    }
+    std::vector<uint2> maps(n_queries);
+    for (uint32_t q = 0; q < n_queries; q++) {
+        const float u = ub[q];
+        if (u > 0.0f && u < INFINITY) {
+            uint32_t bits;
+            memcpy(&bits, &u, 4);
+            maps[q] = uint2{(bits | 0x80000000u) - ((uint32_t)(kDeepBuckets - 1) << 18), 18u};
+        } else {
+            maps[q] = uint2{0u, 24u};
+        }
+    }
+    return maps;
+}
+
 }  // namespace
 
 #define RG_TRY try {
@@ -1846,7 +1886,7 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
     if (!e || !p || !out || (n_queries && !queries) || (n_clauses && !clauses)) throw ArgError("null argument");
     *out = nullptr;
     if (p->k == 0) throw ArgError("k must be >= 1");
-    if (p->k > 1024) throw Unsupported("k > 1024 is not accelerated");
+    if (p->k > kDeepMaxK) throw Unsupported("k > 16384 is not accelerated");
     if (p->mode != RG_MODE_SEARCH && p->mode != RG_MODE_SEARCH_PARALLEL) throw ArgError("bad mode");
     if (e->segs.empty()) throw ArgError("no segment uploaded");
     RG_CUDA_CHECK(cudaSetDevice(e->device));
@@ -1893,6 +1933,9 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
     b->or_has_msm = hp.or_has_msm;
     b->or_has_dmax = hp.or_has_dmax;
     b->n_leaves = (uint32_t)e->segs.size();
+    const bool deep = p->k > 1024u;
+    std::vector<uint2> deep_maps;
+    if (deep) deep_maps = deep_bucket_maps(e, hp, n_queries, p->k1);
     b->postings = hp.postings;
     b->algo_bytes = hp.algo_bytes + (uint64_t)n_queries * p->k * sizeof(rg_hit);
     cudaStream_t st = e->stream;
@@ -1923,8 +1966,10 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
     carve(b->and_grp_ids, hp.and_grp_ids.size());
     carve(b->ro_grp_ids, hp.ro_grp_ids.size());
     // running top-k scores of every OR work item (theta inheritance along a heap chain); skipped when it would
-    // not fit comfortably (huge batches with k near 1024): theta then falls back to the per-range bound
-    b->topk_cap = (std::min<uint32_t>(p->k, 1024u) + 31u) & ~31u;
+    // not fit comfortably (huge batches with k near 1024): theta then falls back to the per-range bound.  Deep
+    // batches keep a score histogram of every item there instead (1 KB each)
+    b->topk_cap = deep ? (uint32_t)kDeepBuckets : (std::min<uint32_t>(p->k, 1024u) + 31u) & ~31u;
+    if (deep) carve(b->deep_map, n_queries);
     const size_t topk_floats = (size_t)b->n_items * b->topk_cap;
     const bool keep_topk = topk_floats * sizeof(float) <= (2ull << 30);
     carve(b->item_topk, keep_topk ? topk_floats : 1);
@@ -1971,6 +2016,7 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
     rebase(b->range_refs); rebase(b->and_rng_ids); rebase(b->ro_rng_ids); rebase(b->range_stats);
     rebase(b->and_grp_ids); rebase(b->ro_grp_ids); rebase(b->group_stats);
     if (p->mode == RG_MODE_SEARCH_PARALLEL) rebase(b->leaf_records);
+    if (deep) rebase(b->deep_map);
     b->zero_begin = b->slab.p + zero_off;
     b->zero_bytes = off - zero_off;
     float* local_base = reinterpret_cast<float*>(b->local_lists.p);
@@ -1992,6 +2038,7 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
     up(b->ro_rng_ids, hp.ro_rng_ids, cs);
     up(b->and_grp_ids, hp.and_grp_ids, cs);
     up(b->ro_grp_ids, hp.ro_grp_ids, cs);
+    if (deep) up(b->deep_map, deep_maps, cs);
     RG_CUDA_CHECK(cudaEventCreateWithFlags(&b->uploaded, cudaEventDisableTiming));
     RG_CUDA_CHECK(cudaEventCreateWithFlags(&b->done, cudaEventDisableTiming));
     for (auto& x : b->ev) RG_CUDA_CHECK(cudaEventCreate(&x));
@@ -2089,6 +2136,7 @@ int rg_batch_run(rg_engine* e, rg_batch* b) {
     ep.error_flag = reinterpret_cast<uint32_t*>(b->arena_next.p + 1);
     ep.dbg = (e->cfg.flags & RG_CFG_STATS) ? b->dbg.p : nullptr;
     ep.touched = b->dbg.p + 15;
+    ep.deep_map = b->k > 1024u ? b->deep_map.p : nullptr;
     RG_CUDA_CHECK(cudaEventRecord(b->ev[2], st));
     ep.cols = b->col_refs.p;
     bool has_live = false, has_other = false;
@@ -2327,7 +2375,7 @@ int rg_batch_leaf_records(rg_engine* e, rg_batch* b, void** dev_ptr, size_t* rec
 
 // finish_parallel on the device into the engine's merge scratch; nothing is copied back and nothing waits
 static void merge_on_device(rg_engine* e, const void* dev_records_all, uint32_t n_leaves, uint32_t n_queries, uint32_t k) {
-    if (k == 0 || k > 1024) throw ArgError("k out of range");
+    if (k == 0 || k > kDeepMaxK) throw ArgError("k out of range");
     RG_CUDA_CHECK(cudaSetDevice(e->device));
     cudaStream_t st = e->stream;
     // grow-only engine scratch: no cudaMalloc/cudaFree on the per-batch path
@@ -2391,6 +2439,7 @@ int rg_batch_rescore(rg_engine* e, rg_batch* b, const rg_query* queries, uint32_
     if (b->generation != e->generation)
         throw ArgError("stale batch: a segment was uploaded or a norm cache changed after rg_batch_prepare");
     if (n_queries != b->n_queries) throw ArgError("rg_batch_rescore: n_queries differs from the batch's");
+    if (b->k > 1024) throw Unsupported("rows of more than 1024 hits are not accelerated");
     RG_CUDA_CHECK(cudaSetDevice(e->device));
     RescorePlan rp;
     plan_rescore(e, queries, n_queries, clauses, n_clauses, rp);
