@@ -57,23 +57,38 @@ struct SegDev {
 // ------------------------------------------------------------------ plan (device side)
 enum : uint32_t { kTypeOr = 0, kTypeAnd = 1, kTypeReqOpt = 2, kTypeDpq = 3 };
 
+// ItemClause::flags, written by the planner (search.cu) and read by the evaluation kernels
+constexpr uint32_t kClauseNot = 1u << 0;       // MUST_NOT clause (ReqNotScorer: excludes, never scores)
+constexpr uint32_t kClauseOpt = 1u << 1;       // SHOULD clause beside a MUST (ReqOptScorer's optional side)
+constexpr uint32_t kClauseColumn = 1u << 2;    // score column: term_id indexes EvalParams::cols
+constexpr uint32_t kClauseTie = 1u << 3;       // meta entry after a DisjunctionMaxScorer item's clauses: weight = tie breaker
+constexpr uint32_t kClauseNoBound = 1u << 4;   // no usable score bound: weight < 0 / NaN or a norm cache with negative entries
+constexpr uint32_t kClauseBitmap = 1u << 5;    // block stream of a term with a presence bitmap: the reference indexes
+                                               // EvalParams::cols (.bits, tf-norm planes)
+constexpr uint32_t kClauseAllDocs = 1u << 6;   // with kClauseColumn: every docid present, cells all 0 (MatchAllDocsQuery)
+constexpr uint32_t kClauseList = 1u << 7;      // block stream read from a scored list: the reference indexes EvalParams::cols (.col)
+constexpr uint32_t kClauseRange = 1u << 8;     // point range: term_id indexes RangeParams::ranges (k_eval_and_ranges / _nested)
+constexpr uint32_t kClauseReqGroup = 1u << 9;  // member of a required pure-SHOULD group (k_eval_and_nested); a group's
+constexpr uint32_t kClauseOptGroup = 1u << 10; // ... or of an optional one; members are contiguous, in member order
+constexpr uint32_t kClauseGroupLast = 1u << 11;  // the last member of its group
+constexpr uint32_t kClauseRefShift = 16;       // bits [16, 32): the EvalParams::cols reference of kClauseBitmap / kClauseList
+
+// WorkItem::type: bits [0, 2) the kType* of the item, bit 2 a DisjunctionMaxScorer item (its tie breaker rides in a
+// kClauseTie entry after the clauses), bits [4, 8) min_should_match when > 1 (kTypeOr only)
+constexpr uint32_t kItemDismax = 1u << 2;
+constexpr uint32_t kItemMsmShift = 4;
+
 struct ItemClause {
     uint32_t term_id;
     float weight;      // idf * boost
     uint32_t cache_id;
-    uint32_t flags;    // bit0: MUST_NOT clause (ReqNotScorer: excludes, never scores)
-                       // bit1: SHOULD clause beside a MUST (ReqOptScorer's optional side)
-                       // bit2: score column — term_id is an index into EvalParams::cols
-                       // bit4: no usable score bound: weight < 0 / NaN or a norm cache with negative entries
-                       // bit5: block stream of a term that has a presence bitmap: bits [16, 32) index EvalParams::cols (.bits)
-                       // bit3: meta entry after a DisjunctionMaxScorer item's clauses: weight = tie breaker
-                       // bit8: point range — term_id indexes RangeParams::ranges (k_eval_and_ranges only)
+    uint32_t flags;    // kClause* bits
 };
 
 struct WorkItem {
     uint32_t query;
     uint16_t seg;
-    uint8_t type;
+    uint8_t type;      // kType* | kItemDismax | msm << kItemMsmShift
     uint8_t n_terms;
     int32_t lo, hi;          // docid range [lo, hi) inside the segment
     uint32_t clause_begin;   // into ItemClause[]
@@ -89,7 +104,7 @@ struct RangeBlock {
     uint32_t docs;      // docids of the block with at least one value
     uint32_t values;    // keys of the block
 };
-// one range clause in one leaf (ItemClause flag bit8: term_id indexes RangeParams::ranges)
+// one range clause in one leaf (an ItemClause with kClauseRange: term_id indexes RangeParams::ranges)
 struct RangeRef {
     const uint32_t* offsets;
     const void* keys;  // uint32_t (wide == 0) or uint64_t (wide == 1)

@@ -109,7 +109,7 @@ k_eval_dpq(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, 
     const SegDev seg = p.segs[it.seg];
     const int T = it.n_terms;
     float* cscores = reinterpret_cast<float*>(cdocs + T * kBlock);
-    const bool dmax_item = (it.type & 4u) != 0;
+    const bool dmax_item = (it.type & kItemDismax) != 0;
     const float tie = dmax_item ? p.clauses[it.clause_begin + T].weight : 0.0f;
     const int lo = 0, hi = seg.max_doc;
 

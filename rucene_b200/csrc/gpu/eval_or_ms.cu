@@ -122,7 +122,7 @@ k_eval_or_ms(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids
     ItemClause c{};
     if (lane < T) {
         c = p.clauses[it.clause_begin + lane];
-        kind = (c.flags & 4u) ? kKindCol : (c.flags & 32u) ? kKindBStream : kKindSparse;
+        kind = (c.flags & kClauseColumn) ? kKindCol : (c.flags & kClauseBitmap) ? kKindBStream : kKindSparse;
     }
     const uint32_t col_mask = __ballot_sync(0xffffffffu, kind == kKindCol);
     const uint32_t bstream_mask = __ballot_sync(0xffffffffu, kind == kKindBStream);
@@ -158,7 +158,7 @@ k_eval_or_ms(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids
         sh.bits[lane] = nullptr;
         sh.hi1[lane] = sh.hi2[lane] = nullptr;
         if (kind == kKindBStream) {
-            const ColRef r = p.cols[c.flags >> 16];
+            const ColRef r = p.cols[c.flags >> kClauseRefShift];
             sh.bits[lane] = r.bits;
             sh.hi1[lane] = r.hi1;
             sh.hi2[lane] = r.hi2;
@@ -172,7 +172,7 @@ k_eval_or_ms(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids
         const float w1 = __fmul_rn(c.weight, __fadd_rn(p.k1, 1.0f));
         // score = rn(rn(w1*f) / rn(f + norm)) with f >= 1, norm >= 0  =>  score <= nextafter(w1); with a tf-norm factor
         // (rounded up at build time) <= tau:  score <= w1 * tau * (1 + 4 * 2^-24)
-        ub = (c.flags & 16u) || !(w1 >= 0.0f) || !(w1 < INFINITY) ? INFINITY : __uint_as_float(__float_as_uint(w1) + 1u);
+        ub = (c.flags & kClauseNoBound) || !(w1 >= 0.0f) || !(w1 < INFINITY) ? INFINITY : __uint_as_float(__float_as_uint(w1) + 1u);
         const bool planes = PLANES && sh.hi1[lane] != nullptr && ub < INFINITY;
         ub0 = planes ? fminf(ub, __fmul_ru(__fmul_ru(w1, tau1), 1.000001f)) : ub;
         ub1 = planes ? fminf(ub, __fmul_ru(__fmul_ru(w1, tau2), 1.000001f)) : ub;

@@ -277,15 +277,15 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
     for (int i = lane; i < kWw; i += 32) sh.acc[i] = POS ? 0u : kSent;
     MsmCtx mc;
     mc.cnt = reinterpret_cast<uint8_t*>(cscores + T * kBlock);  // MSM variants reserve kWw more bytes
-    mc.msm = max(1u, (uint32_t)it.type >> 4);  // items without min_should_match in an MSM launch: 1
+    mc.msm = max(1u, (uint32_t)it.type >> kItemMsmShift);  // items without min_should_match in an MSM launch: 1
     mc.mx = reinterpret_cast<float*>(mc.cnt + kWw);  // DMAX variant reserves 4 * kWw more bytes
     // DisjunctionMaxScorer item: the tie breaker rides in a meta clause after the item's clauses
-    const bool dmax_item = DMAX && (it.type & 4u) != 0;
+    const bool dmax_item = DMAX && (it.type & kItemDismax) != 0;
     const float tie = dmax_item ? p.clauses[it.clause_begin + T].weight : 0.0f;
     if (MSM) {
         for (int i = lane; i < kWw / 4; i += 32) reinterpret_cast<uint32_t*>(mc.cnt)[i] = 0u;
     }
-    if (lane < T && (p.clauses[it.clause_begin + lane].flags & 4u)) {
+    if (lane < T && (p.clauses[it.clause_begin + lane].flags & kClauseColumn)) {
         // score column (a hot, dense clause whose BM25 contributions were materialised once for the
         // whole batch): no stream; the column is read window by window
         const ItemClause c = p.clauses[it.clause_begin + lane];
@@ -300,14 +300,14 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
         tc.term_id = c.term_id;
         tc.w1 = 0.0f;
         tc.is_not = 0;
-        tc.is_col = (c.flags & 64u) ? 2 : 1;  // 2: every docid present (MatchAllDocsQuery), cells all 0
+        tc.is_col = (c.flags & kClauseAllDocs) ? 2 : 1;  // 2: every docid present (MatchAllDocsQuery), cells all 0
         tc.col_dbg = LEAN ? p.dbg : nullptr;
     } else if (lane < T) {
         const ItemClause c = p.clauses[it.clause_begin + lane];
         const TermDev td = seg.terms[c.term_id];
         WTerm& tc = sh.term[lane];
         tc.is_col = 0;
-        tc.pre = (c.flags & 128u) ? reinterpret_cast<const uint4*>(p.cols[c.flags >> 16].col) : nullptr;
+        tc.pre = (c.flags & kClauseList) ? reinterpret_cast<const uint4*>(p.cols[c.flags >> kClauseRefShift].col) : nullptr;
         tc.blk_last = seg.blk_last + td.blk_begin;
         tc.blk_desc = seg.blk_desc + td.blk_begin;
         tc.cache = p.caches + (size_t)c.cache_id * 256;
@@ -317,7 +317,7 @@ k_eval_or(EvalParams p, const uint32_t* __restrict__ item_ids, uint32_t n_ids, u
         tc.pos = 0;
         tc.term_id = c.term_id;
         tc.w1 = __fmul_rn(c.weight, __fadd_rn(p.k1, 1.0f));
-        tc.is_not = c.flags & 1u;
+        tc.is_not = c.flags & kClauseNot;
     }
     __syncwarp();
     const bool my_stream = lane < T && sh.term[lane < T ? lane : 0].is_col == 0;  // lane t: clause t is not a column
@@ -602,7 +602,7 @@ struct AndSharedR : AndShared {
     uint32_t rcur;             // next lead block to look at
 };
 
-// k_eval_and_nested: pure-SHOULD groups of terms (ItemClause bits 9-11).  A group that leads keeps each member's
+// k_eval_and_nested: pure-SHOULD groups of terms (kClauseReqGroup / kClauseOptGroup / kClauseGroupLast).  A group that leads keeps each member's
 // current decoded block here (one member per warp; apart from slab_docs, which the probes overwrite every step); a
 // group probed after the lead sums its members per slot in gsum.
 struct AndSharedN : AndSharedR {
@@ -614,7 +614,7 @@ struct AndSharedN : AndSharedR {
     int32_t gn[kEvalWarps];             // entries in the slab
     uint32_t gblk[kEvalWarps];          // next block to decode (nb = the vint tail / singleton)
     uint32_t gdone[kEvalWarps];         // no block left in [lo, hi)
-    uint32_t grp[kMaxTerms];            // ItemClause bits 9-11 of each clause
+    uint32_t grp[kMaxTerms];            // the group bits of each clause's flags
     int32_t gx;                         // this step merges docids from gx on
 };
 
@@ -632,9 +632,9 @@ __device__ __forceinline__ bool range_hit(const RangeRef& r, int d) {
 }
 
 // OTHER: some leaf carries EF / BITSET doc blocks (their decoder is compiled out otherwise).
-// RANGES: the item has point-range clauses (ItemClause bit8); a range that leads walks the item's docids one 128-doc
+// RANGES: the item has point-range clauses (kClauseRange); a range that leads walks the item's docids one 128-doc
 // block per warp.  Without it the body is the plain conjunction / ReqOpt kernel, unchanged.
-// GROUPS: the item has pure-SHOULD groups of terms (ItemClause bits 9-11, see AndSharedN); a group that leads merges
+// GROUPS: the item has pure-SHOULD groups of terms (kClauseReqGroup / kClauseOptGroup, see AndSharedN); a group that leads merges
 // its members' postings in docid order.  gstats: group-lead counters (GROUPS only).
 // DEEP: k > kMaxK — theta from a score histogram in EmitShared::topk (see deep_publish).
 template <bool REQOPT, bool OTHER, bool RANGES, bool GROUPS = false, bool DEEP = false>
@@ -654,18 +654,18 @@ __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_
     emit_init(sh.emit);
     if ((int)threadIdx.x < T) {
         const ItemClause c = p.clauses[it.clause_begin + threadIdx.x];
-        const bool is_col = (c.flags & 4u) != 0;  // term_id indexes p.cols then (never the lead clause)
-        const bool is_rng = RANGES && (c.flags & 256u) != 0;  // term_id indexes rp.ranges
+        const bool is_col = (c.flags & kClauseColumn) != 0;  // term_id indexes p.cols then (never the lead clause)
+        const bool is_rng = RANGES && (c.flags & kClauseRange) != 0;  // term_id indexes rp.ranges
         if (RANGES) {
             shr.is_rng[threadIdx.x] = is_rng;
             if (is_rng) shr.rref[threadIdx.x] = rp.ranges[c.term_id];
         }
-        if (GROUPS) shn.grp[threadIdx.x] = c.flags & (512u | 1024u | 2048u);
+        if (GROUPS) shn.grp[threadIdx.x] = c.flags & (kClauseReqGroup | kClauseOptGroup | kClauseGroupLast);
         const TermDev td = (is_col || is_rng) ? TermDev{} : seg.terms[c.term_id];
         TermCtx& tc = sh.term[threadIdx.x];
         sh.term_id[threadIdx.x] = c.term_id;
-        sh.is_not[threadIdx.x] = c.flags & 1u;
-        sh.is_opt[threadIdx.x] = (c.flags >> 1) & 1u;
+        sh.is_not[threadIdx.x] = c.flags & kClauseNot;
+        sh.is_opt[threadIdx.x] = (c.flags / kClauseOpt) & 1u;
         sh.colp[threadIdx.x] = is_col ? p.cols[c.term_id].col : nullptr;
         tc.blk_last = seg.blk_last + td.blk_begin;
         tc.blk_desc = seg.blk_desc + td.blk_begin;
@@ -700,10 +700,10 @@ __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_
     unsigned long long rstat[3] = {0ull, 0ull, 0ull};  // range-lead blocks skipped / whole / scanned (lane 0s)
     // a group leads when its first member is clause 0; its members are clauses [0, G)
     int G = 1;
-    const bool group_lead = GROUPS && (shn.grp[0] & 512u) != 0;
+    const bool group_lead = GROUPS && (shn.grp[0] & kClauseReqGroup) != 0;
     if (GROUPS && group_lead) {
         G = 0;
-        while (!(shn.grp[G] & 2048u)) G++;
+        while (!(shn.grp[G] & kClauseGroupLast)) G++;
         G++;
         if (warp < G && lane == 0) {
             shn.gblk[warp] = sh.term[warp].cur;
@@ -1133,10 +1133,10 @@ __device__ __forceinline__ void eval_and_body(const EvalParams& p, const uint32_
                 }
             }
             __syncwarp();
-            if (GROUPS && (shn.grp[t] & 2048u)) {
+            if (GROUPS && (shn.grp[t] & kClauseGroupLast)) {
                 // after a group's last member: a required group drops a slot none of its members matched and adds
                 // its sum (one f32 value) to the conjunction's; an optional one adds its sum to the optional side's
-                const bool greq = (shn.grp[t] & 512u) != 0;
+                const bool greq = (shn.grp[t] & kClauseReqGroup) != 0;
 #pragma unroll
                 for (int r = 0; r < kAndSteps; r++) {
                     const int slot = warp * kBlock + r * 32 + lane;

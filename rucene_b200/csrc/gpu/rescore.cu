@@ -69,7 +69,7 @@ __device__ void probe_clause(const RescoreParams& p, const SegDev& seg, const It
     const uint32_t nb = td.n_blocks;
     const float w1 = __fmul_rn(c.weight, __fadd_rn(p.k1, 1.0f));
     const float* cache = p.caches + (size_t)c.cache_id * 256;
-    const uint32_t role = c.flags & 3u;  // 0 required / scoring, 1 MUST_NOT, 2 optional
+    const uint32_t role = c.flags & (kClauseNot | kClauseOpt);  // 0 required / scoring, kClauseNot, kClauseOpt
     const int base = seg.doc_base;
     uint32_t pos = b, hint = 0;
     while (pos < e) {
@@ -115,9 +115,9 @@ __device__ void probe_clause(const RescoreParams& p, const SegDev& seg, const It
                 if (l < n_in && bdocs[l] == dj) {
                     const float nrm = seg.norms ? __ldg(cache + __ldg(seg.norms + dj)) : p.k1;
                     const float s = bm25_score(w1, (float)bfreqs[l], nrm);
-                    if (role == 1u) {
+                    if (role == kClauseNot) {
                         st[j] |= kRsExcl;
-                    } else if (role == 2u) {
+                    } else if (role == kClauseOpt) {
                         acc2[j] = __fadd_rn(acc2[j], s);  // DisjunctionSumScorer from 0.0f, clause order
                         st[j] |= kRsOptAny;
                     } else if (kind == kRsTerm) {

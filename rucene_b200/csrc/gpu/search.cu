@@ -33,11 +33,29 @@ struct Span {
     size_t bytes() const { return n * sizeof(T); }
 };
 
+// The kernel routes of work items: each route is one launch list of rg_batch_run.
+enum Route : uint32_t {
+    kRouteOr,            // k_eval_or over block streams (any disjunction k_eval_or_ms and the decode-free one do not take)
+    kRouteMs,            // k_eval_or_ms: plain sums with presence bitmaps; non-essential clauses are only counted
+    kRouteLean,          // the decode-free k_eval_or: every clause a score column or a scored list
+    kRouteDpq,           // k_eval_dpq: >= 10 clauses in the leaf (DisiPriorityQueue), one item per (query, leaf)
+    kRouteAnd,           // k_eval_and: conjunctions
+    kRouteReqOpt,        // k_eval_and<REQOPT>: MUST + SHOULD (ReqOptScorer)
+    kRouteAndRanges,     // k_eval_and_ranges: conjunctions with a point-range clause
+    kRouteReqOptRanges,
+    kRouteAndNested,     // k_eval_and_nested: conjunctions with a group member (ranges or not)
+    kRouteReqOptNested,
+    kRoutes
+};
+// Routes whose items launch range-major (all first docid ranges, then all second ones, ...: see plan_batch); the
+// others launch in item order (their items mostly cover a whole leaf: a ReqOptScorer's running mean, the
+// DisiPriorityQueue).
+constexpr bool kRouteByRank[kRoutes] = {true, true, true, false, true, false, true, false, true, false};
+
 struct rg_batch {
     uint32_t n_queries = 0, k = 0, mode = 0;
     float k1 = 1.2f;
-    uint32_t n_items = 0, n_or = 0, n_ms = 0, n_and = 0, n_ro = 0, n_groups = 0, n_leaves = 0, max_or_terms = 1,
-             max_ms_streams = 0;
+    uint32_t n_items = 0, n_groups = 0, n_leaves = 0;
     uint64_t generation = 0;  // engine->generation at prepare time
     // One device allocation per batch (cudaMalloc/cudaFree cost milliseconds each next to a
     // multi-GB index image; the engine keeps the last slab for the next batch).  Layout:
@@ -45,15 +63,11 @@ struct rg_batch {
     DevBuf<uint8_t> slab;
     Span<WorkItem> items;
     Span<ItemClause> clauses;
-    Span<uint32_t> or_ids, and_ids;  // launch order (range-major) of the OR / AND work items
-    Span<uint32_t> ms_ids;           // OR work items evaluated by k_eval_or_ms (bitmaps + non-essential clauses)
-    Span<uint32_t> lean_ids;         // OR work items of the decode-free k_eval_or (every clause a column / scored list)
-    uint32_t n_lean = 0;
+    Span<uint32_t> ids[kRoutes];     // the work items of each route, in launch order
+    uint32_t n_ids[kRoutes] = {};
+    uint32_t width[kRoutes] = {};    // widest item of k_eval_or / k_eval_dpq (clauses) and k_eval_or_ms (block streams)
     Span<uint4> local_lists;         // batch-local scored lists (choose_local_lists), built by rg_batch_prepare
-    Span<uint32_t> dpq_ids;          // disjunctions with >= 10 clauses in the leaf (k_eval_dpq), one per (query, leaf)
-    uint32_t n_dpq = 0, max_dpq_terms = 0;
     bool uses_planes = false;        // some column / bitmap reference of this batch carries tf-norm planes
-    Span<uint32_t> ro_ids;           // MUST+SHOULD (ReqOptScorer) work items: one per (query, leaf)
     Span<ColRef> col_refs;           // score columns this batch reads (ItemClause.term_id indexes it)
     std::vector<std::shared_ptr<ColEntry>> cols;  // keeps them alive (the engine's LRU may drop them meanwhile)
     std::vector<std::shared_ptr<ColEntry>> lists; // scored posting lists this batch streams, likewise
@@ -83,15 +97,10 @@ struct rg_batch {
     cudaEvent_t uploaded = nullptr, done = nullptr, ev[4] = {nullptr, nullptr, nullptr, nullptr};
     bool synced = false;  // the host has waited for `done`
     DevBuf<uint8_t> rescore_plan;  // the last rg_batch_rescore's plan (read by its k_rescore)
-    // point ranges: RangeRef per (leaf, range), the items of k_eval_and_ranges, its block counters (zeroed per run)
+    // point ranges: RangeRef per (leaf, range) and the range kernels' block counters (zeroed per run)
     Span<RangeRef> range_refs;
-    Span<uint32_t> and_rng_ids, ro_rng_ids;
-    uint32_t n_and_rng = 0, n_ro_rng = 0;
     Span<unsigned long long> range_stats;
-    // nested groups: the items of k_eval_and_nested and its group-lead counters (zeroed per run)
-    Span<uint32_t> and_grp_ids, ro_grp_ids;
-    uint32_t n_and_grp = 0, n_ro_grp = 0;
-    Span<unsigned long long> group_stats;
+    Span<unsigned long long> group_stats;  // group-lead counters of k_eval_and_nested (zeroed per run)
     ~rg_batch() {
         for (cudaEvent_t x : {uploaded, done, ev[0], ev[1], ev[2], ev[3]})
             if (x) cudaEventDestroy(x);
@@ -121,12 +130,10 @@ struct PlanTimer {
 struct HostPlan {
     std::vector<WorkItem> items;
     std::vector<ItemClause> clauses;
-    std::vector<uint32_t> or_ids, ms_ids, and_ids, ro_ids, dpq_ids, lean_ids;
-    uint32_t max_dpq_terms = 0;
-    // point ranges: RangeRef per (leaf, range); conjunction / ReqOpt items with a range clause (k_eval_and_ranges)
-    std::vector<RangeRef> range_refs;
-    std::vector<uint32_t> and_rng_ids, ro_rng_ids;
-    std::vector<uint32_t> and_grp_ids, ro_grp_ids;  // conjunction / ReqOpt items with a group (k_eval_and_nested)
+    std::vector<uint32_t> ids[kRoutes];   // the work items of each route
+    std::vector<uint32_t> rank[kRoutes];  // kRouteByRank routes: the launch-order key of each id
+    uint32_t width[kRoutes] = {};
+    std::vector<RangeRef> range_refs;     // point ranges: RangeRef per (leaf, range)
     // batch-local scored lists: build jobs whose dst is an offset (in floats) into the batch's list region, and the
     // col_refs entries to point there once the slab exists
     std::vector<ColumnJob> local_jobs;
@@ -136,26 +143,26 @@ struct HostPlan {
     std::vector<ColRef> col_refs;
     std::map<std::tuple<uint32_t, uint32_t, uint32_t>, uint32_t> bitmap_refs;  // (leaf, term, cache) -> col_refs entry {null, bits, hi}
     std::vector<std::shared_ptr<ColEntry>> cols, lists;
-    uint32_t n_cols_built = 0, n_lists_built = 0, max_ms_streams = 0;
+    uint32_t n_cols_built = 0, n_lists_built = 0;
     uint64_t col_floats = 0, list_floats = 0;
-    std::vector<uint32_t> or_rank, ms_rank, and_rank, lean_rank;  // range index of each id (launch-order key)
     std::vector<uint32_t> group_item_begin, group_out;
     uint64_t postings = 0, algo_bytes = 0;
-    uint32_t max_or_terms = 1;
     bool or_has_not = false, or_has_msm = false, or_has_dmax = false, or_nonpos = false;
     // back to the empty plan, keeping the vectors' storage (a plan is tens of MB: fresh vectors would be page-faulted
     // in by every rg_batch_prepare)
     void reset() {
-        items.clear(); clauses.clear(); or_ids.clear(); ms_ids.clear(); and_ids.clear(); ro_ids.clear(); dpq_ids.clear();
-        lean_ids.clear(); lean_rank.clear(); local_jobs.clear(); local_refs.clear();
-        range_refs.clear(); and_rng_ids.clear(); ro_rng_ids.clear(); and_grp_ids.clear(); ro_grp_ids.clear();
+        items.clear(); clauses.clear(); local_jobs.clear(); local_refs.clear(); range_refs.clear();
+        for (uint32_t r = 0; r < kRoutes; r++) {
+            ids[r].clear();
+            rank[r].clear();
+            width[r] = 0;
+        }
         local_floats = 0;
         local_units = 0;
-        col_refs.clear(); bitmap_refs.clear(); cols.clear(); lists.clear(); or_rank.clear(); ms_rank.clear(); and_rank.clear();
+        col_refs.clear(); bitmap_refs.clear(); cols.clear(); lists.clear();
         group_item_begin.clear(); group_out.clear();
-        max_dpq_terms = n_cols_built = n_lists_built = max_ms_streams = 0;
+        n_cols_built = n_lists_built = 0;
         col_floats = list_floats = postings = algo_bytes = 0;
-        max_or_terms = 1;
         or_has_not = or_has_msm = or_has_dmax = or_nonpos = false;
     }
 };
@@ -178,18 +185,29 @@ struct QShape {
     // point ranges (RG_CLAUSE_RANGE, only from the *_ranges entry points): required (MUST / FILTER, or the one clause
     // a query collapses to) and MUST_NOT ones.  A shape with ranges is always kTypeAnd or kTypeReqOpt.
     std::vector<uint32_t> req_rng, not_rng;
-    // nested groups (RG_CLAUSE_GROUP, only from the *_nested entry points) of a conjunction / ReqOpt shape: the
-    // required side (MUST then FILTER) and the optional side in clause order, terms and groups mixed.  clause_idx /
-    // opt_idx still list the terms among them (columns are chosen from those); not_idx holds MUST_NOT groups flattened.
+    // What a kTypeAnd / kTypeReqOpt shape is planned from: the required side (MUST then FILTER) and the optional side,
+    // in clause order, terms and nested groups (RG_CLAUSE_GROUP, only from the *_nested entry points) mixed.
+    // clause_idx / opt_idx list the terms among them (columns are chosen from those); not_idx holds MUST_NOT groups
+    // flattened.
     struct Entry {
+        uint32_t begin, n;  // its clauses [begin, begin + n): a term's one clause, or a group's members
         bool group;
-        uint32_t ci;        // a term: its clause
-        uint32_t begin, n;  // a group: member clauses [begin, begin + n)
         bool filter;        // a FILTER group: needs_scores = false, it scores exactly 0.0f
     };
-    bool nested = false;
     std::vector<Entry> req_seq, opt_seq;
+    // a shape without groups: every required / optional clause is a term entry
+    void term_entries() {
+        for (uint32_t ci : clause_idx) req_seq.push_back(Entry{ci, 1, false, false});
+        for (uint32_t ci : opt_idx) opt_seq.push_back(Entry{ci, 1, false, false});
+    }
 };
+
+// MUST_NOT clauses never score, but the kernels still form cache pointers from the id
+void check_caches(const QShape& s, const rg_clause* clauses, uint32_t n_caches) {
+    for (const auto* idx : {&s.clause_idx, &s.opt_idx, &s.not_idx})
+        for (uint32_t ci : *idx)
+            if (clauses[ci].cache_id >= n_caches) throw ArgError("clause refers to an unset norm cache");
+}
 
 inline bool is_range_clause(const rg_clause& c, const rg_point_range* ranges) {
     return ranges && (c.occur & RG_CLAUSE_RANGE);
@@ -258,6 +276,7 @@ bool classify_ranges(const rg_query& q, const rg_clause* clauses, const rg_point
     s.clause_idx = req_terms;
     s.opt_idx = shoulds;
     s.not_idx = must_nots;
+    s.term_entries();
     return true;
 }
 
@@ -342,6 +361,7 @@ QShape classify(const rg_query& q, const rg_clause* clauses, uint32_t n_clauses_
         s.type = shoulds.empty() ? kTypeAnd : kTypeReqOpt;
         s.clause_idx = musts;
         s.opt_idx = shoulds;
+        s.term_entries();
         return s;
     }
     s.type = kTypeOr;
@@ -419,22 +439,20 @@ bool classify_groups(const rg_query& q, std::vector<rg_clause>& ext, uint32_t n_
             (occ == RG_MUST_NOT ? s.not_rng : occ == RG_SHOULD ? should_rng : s.req_rng).push_back(ci);
             continue;
         }
-        Entry e{false, ci, 0, 0, false};
+        Entry e{ci, 1, false, false};
         if (grp) {
             const rg_query& g = groups[c.term_id];
             if (g.n_clauses == 1) {  // a group of one clause is that clause
                 const rg_clause& m = ext[g.clause_begin];
-                e.ci = (uint32_t)ext.size();
+                e.begin = (uint32_t)ext.size();
                 ext.push_back(rg_clause{occ, m.term_id, m.weight, m.cache_id});
             } else {
-                e = Entry{true, 0, g.clause_begin, g.n_clauses, occ == RG_FILTER};
+                e = Entry{g.clause_begin, g.n_clauses, true, occ == RG_FILTER};
             }
         }
-        n_flat += e.group ? e.n : 1;
+        n_flat += e.n;
         if (occ == RG_MUST_NOT) {
-            if (e.group)
-                for (uint32_t j = 0; j < e.n; j++) nots.push_back(e.begin + j);
-            else nots.push_back(e.ci);
+            for (uint32_t j = 0; j < e.n; j++) nots.push_back(e.begin + j);
         } else {
             (occ == RG_MUST ? musts : occ == RG_FILTER ? filters : shoulds).push_back(e);
         }
@@ -466,7 +484,7 @@ bool classify_groups(const rg_query& q, std::vector<rg_clause>& ext, uint32_t n_
             lone_group(e);
         } else {
             s.type = kTypeOr;
-            s.clause_idx.push_back(e.ci);
+            s.clause_idx.push_back(e.begin);
         }
         return true;
     }
@@ -487,15 +505,14 @@ bool classify_groups(const rg_query& q, std::vector<rg_clause>& ext, uint32_t n_
         s.not_idx = nots;
         return true;
     }
-    s.nested = true;
     s.type = shoulds.empty() ? kTypeAnd : kTypeReqOpt;
     s.req_seq = musts;
     s.req_seq.insert(s.req_seq.end(), filters.begin(), filters.end());
     s.opt_seq = shoulds;
     for (const Entry& e : s.req_seq)
-        if (!e.group) s.clause_idx.push_back(e.ci);
+        if (!e.group) s.clause_idx.push_back(e.begin);
     for (const Entry& e : s.opt_seq)
-        if (!e.group) s.opt_idx.push_back(e.ci);
+        if (!e.group) s.opt_idx.push_back(e.begin);
     s.not_idx = nots;
     return true;
 }
@@ -581,6 +598,34 @@ bool resolve_ranges(const QShape& shape, const Segment& seg, const rg_clause* cl
 // batch share it (RG_CFG_EAGER_COLUMNS: one), most valuable (uses x df) first, evicting least recently
 // used columns no batch references while over the HBM budget.  RG_CFG_NO_COLUMNS turns the feature off.
 constexpr uint32_t kMatchAllTerm = 0xffffffffu;  // ColKey term of a leaf's MatchAllDocsQuery column
+
+// the score column / scored list of a clause in leaf si
+ColKey col_key(uint32_t si, const rg_clause& c, uint32_t k1bits) {
+    const float w = clause_weight(c);
+    uint32_t wbits;
+    memcpy(&wbits, &w, 4);
+    return ColKey(si, c.term_id, wbits, c.cache_id, k1bits);
+}
+
+// the col_refs entry of a clause's score column in leaf si, -1: none
+int64_t col_of(const std::map<ColKey, uint32_t>& columns, uint32_t si, const rg_clause& c, uint32_t k1bits) {
+    if (columns.empty()) return -1;
+    const auto it = columns.find(col_key(si, c, k1bits));
+    return it == columns.end() ? -1 : (int64_t)it->second;
+}
+
+// the build job of a column or list: its work units (blocks and tail) start at unit_begin of the launch
+ColumnJob column_job(const ColKey& key, void* dst, uint32_t unit_begin) {
+    ColumnJob job{};
+    job.seg = std::get<0>(key);
+    job.term_id = std::get<1>(key);
+    const uint32_t wbits = std::get<2>(key);
+    memcpy(&job.weight, &wbits, 4);
+    job.cache_id = std::get<3>(key);
+    job.dst = dst;
+    job.unit_begin = unit_begin;
+    return job;
+}
 
 // tf-norm planes of a bitmap term for one (norm cache, k1) — see TfPlanes: built for ALL bitmap terms of the leaf the
 // first time a batch asks (a histogram pass over a sample of their blocks picks tau1/tau2, one more pass sets the
@@ -798,11 +843,8 @@ std::map<ColKey, uint32_t> choose_columns(rg_engine* e, const std::vector<QShape
                 const rg_clause& c = clauses[ci];
                 if (c.term_id >= seg.host_terms.size() || seg.bitmap_slot[c.term_id] < 0) return;
                 if ((uint64_t)seg.host_terms[c.term_id].doc_freq * den < (uint64_t)seg.max_doc) return;
-                const float w = clause_weight(c);
-                if (!scores_positive(seg, w, c.cache_id, k1)) return;  // a column cell of +0.0f means "no posting"
-                uint32_t wbits;
-                memcpy(&wbits, &w, 4);
-                uses[ColKey(si, c.term_id, wbits, c.cache_id, k1bits)]++;
+                if (!scores_positive(seg, clause_weight(c), c.cache_id, k1)) return;  // a column cell of +0.0f means "no posting"
+                uses[col_key(si, c, k1bits)]++;
             };
             const uint64_t or_den = ((e->cfg.flags & RG_CFG_MAXSCORE) || eager) ? (uint64_t)kColumnDen : (uint64_t)e->or_col_den;
             for (uint32_t ci : sh.clause_idx) count(ci, sh.type == kTypeOr ? or_den : (uint64_t)kColumnDen);
@@ -882,16 +924,8 @@ std::map<ColKey, uint32_t> choose_columns(rg_engine* e, const std::vector<QShape
         ent->bmax = reinterpret_cast<uint32_t*>(ent->col + col_len);
         built.push_back(ent);
         RG_CUDA_CHECK(cudaMemsetAsync(ent->col, 0, len * sizeof(float), st));
-        ColumnJob job{};
-        job.seg = std::get<0>(r.second);
-        job.term_id = std::get<1>(r.second);
-        const uint32_t wbits = std::get<2>(r.second);
-        memcpy(&job.weight, &wbits, 4);
-        job.cache_id = std::get<3>(r.second);
-        job.dst = ent->col;
-        job.unit_begin = n_units;
+        jobs.push_back(column_job(r.second, ent->col, n_units));
         n_units += th.n_blocks + (th.tail_n ? 1u : 0u);
-        jobs.push_back(job);
         e->col_cache[r.second] = ent;
         e->col_floats += len;
         e->col_builds++;
@@ -944,10 +978,7 @@ std::map<ColKey, uint32_t> choose_lists(rg_engine* e, const std::vector<QShape>&
                 if (c.term_id >= seg.host_terms.size()) continue;
                 const uint64_t df = (uint64_t)seg.host_terms[c.term_id].doc_freq;
                 if (df < min_df) continue;
-                const float w = clause_weight(c);
-                uint32_t wbits;
-                memcpy(&wbits, &w, 4);
-                const ColKey key(si, c.term_id, wbits, c.cache_id, k1bits);
+                const ColKey key = col_key(si, c, k1bits);
                 if (df * e->or_col_den >= (uint64_t)seg.max_doc && columns.count(key)) continue;  // read from its score column
                 uses[key]++;
             }
@@ -1011,16 +1042,8 @@ std::map<ColKey, uint32_t> choose_lists(rg_engine* e, const std::vector<QShape>&
         ent->col = base + pk.off;
         ent->in_arena = true;
         e->list_slabs.back().entries.push_back(ent);
-        ColumnJob job{};
-        job.seg = std::get<0>(pk.key);
-        job.term_id = std::get<1>(pk.key);
-        const uint32_t wbits = std::get<2>(pk.key);
-        memcpy(&job.weight, &wbits, 4);
-        job.cache_id = std::get<3>(pk.key);
-        job.dst = ent->col;
-        job.unit_begin = n_units;
+        jobs.push_back(column_job(pk.key, ent->col, n_units));
         n_units += pk.units;
-        jobs.push_back(job);
         e->list_cache[pk.key] = ent;
         e->list_floats += pk.len;
         e->list_builds++;
@@ -1086,10 +1109,7 @@ void choose_local_lists(rg_engine* e, const std::vector<QShape>& shapes, const r
                 const rg_clause& c = clauses[ci];
                 const uint64_t df = df_of(c);
                 if (!df) continue;
-                const float w = clause_weight(c);
-                uint32_t wbits;
-                memcpy(&wbits, &w, 4);
-                const ColKey key(si, c.term_id, wbits, c.cache_id, k1bits);
+                const ColKey key = col_key(si, c, k1bits);
                 if ((df * e->or_col_den >= (uint64_t)seg.max_doc && columns.count(key)) || lists.count(key)) continue;
                 // + one unit: stream_refill prefetches the block after a full block, and a list whose item keeps a
                 // block stream (budget) is read by the stream variant
@@ -1114,15 +1134,8 @@ void choose_local_lists(rg_engine* e, const std::vector<QShape>& shapes, const r
         lists[key] = (uint32_t)hp.col_refs.size();
         hp.local_refs.emplace_back((uint32_t)hp.col_refs.size(), hp.local_floats);
         hp.col_refs.push_back(ColRef{nullptr, nullptr, nullptr, nullptr, 1.0f, 1.0f});
-        ColumnJob job{};
-        job.seg = std::get<0>(key);
-        job.term_id = std::get<1>(key);
-        const uint32_t wbits = std::get<2>(key);
-        memcpy(&job.weight, &wbits, 4);
-        job.cache_id = std::get<3>(key);
-        job.dst = reinterpret_cast<void*>((uintptr_t)hp.local_floats);  // rebased in rg_batch_prepare
-        job.unit_begin = hp.local_units;
-        hp.local_jobs.push_back(job);
+        // dst is an offset in floats, rebased in rg_batch_prepare
+        hp.local_jobs.push_back(column_job(key, reinterpret_cast<void*>((uintptr_t)hp.local_floats), hp.local_units));
         hp.local_units += th.n_blocks + (th.tail_n ? 1u : 0u);
         hp.local_floats += r.first;
     }
@@ -1135,7 +1148,7 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
     const uint32_t n_caches = (uint32_t)(e->h_caches.size() / 256);
     const uint32_t n_segs = (uint32_t)e->segs.size();
     std::vector<QShape> shapes(n_queries);
-    bool any_ranges = false, any_groups = false;
+    bool any_ranges = false;
     // groups: the clause array grows by what the collapses make (classify_groups)
     std::vector<rg_clause> ext;
     if (groups) ext.assign(clauses, clauses + n_clauses);
@@ -1143,19 +1156,12 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
         if (ranges && (uint64_t)queries[qi].clause_begin + queries[qi].n_clauses > n_clauses)
             throw ArgError("query clause range out of bounds");
         if (groups && classify_groups(queries[qi], ext, n_clauses, ranges, n_ranges, groups, n_groups, n_caches, shapes[qi])) {
-            any_groups = true;
             any_ranges = any_ranges || !shapes[qi].req_rng.empty() || !shapes[qi].not_rng.empty();
         } else if (ranges && classify_ranges(queries[qi], groups ? ext.data() : clauses, ranges, n_ranges, shapes[qi]))
             any_ranges = true;
         else shapes[qi] = classify(queries[qi], groups ? ext.data() : clauses, n_clauses);
         if (groups) clauses = ext.data();  // (ext may have moved)
-        for (uint32_t ci : shapes[qi].clause_idx)
-            if (clauses[ci].cache_id >= n_caches) throw ArgError("clause refers to an unset norm cache");
-        for (uint32_t ci : shapes[qi].opt_idx)
-            if (clauses[ci].cache_id >= n_caches) throw ArgError("clause refers to an unset norm cache");
-        // MUST_NOT clauses never score, but the kernels still form cache pointers from the id
-        for (uint32_t ci : shapes[qi].not_idx)
-            if (clauses[ci].cache_id >= n_caches) throw ArgError("clause refers to an unset norm cache");
+        check_caches(shapes[qi], clauses, n_caches);
     }
     // Docid ranges (= work items) per (query, leaf).  A caller's rg_config.range_postings is taken as is: ~that many
     // postings per range.  By default conjunction items (one CTA each) get 32 K postings; disjunctions (one warp each)
@@ -1220,119 +1226,31 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
     std::mutex refs_mutex;
     const uint32_t n_threads = n_queries >= 512 ? std::min<uint32_t>(16u, std::max(1u, std::thread::hardware_concurrency())) : 1u;
     auto plan_range = [&](uint32_t q_begin, uint32_t q_end, HostPlan& lp) {
+    // a required / optional clause of a conjunction in one leaf: its clauses there are members[begin, begin + n)
+    struct Req {
+        uint64_t cost;
+        uint32_t begin, n;
+        bool group, filter;
+    };
+    // scratch of every (query, leaf) this thread plans
+    std::vector<Req> req, opt;
+    std::vector<uint32_t> members, present, nots, opts, rnots;
+    std::vector<std::pair<uint64_t, uint32_t>> rreq;
     for (uint32_t qi = q_begin; qi < q_end; qi++) {
         const QShape& shape = shapes[qi];
         bool group_open = false;
         uint32_t chain_pos = 0;
         for (uint32_t si = 0; si < n_segs; si++) {
             const Segment& seg = e->segs[si];
-            // resolve clauses against this leaf: present (conjunctions in cost order), MUST_NOT, optional side
-            std::vector<uint32_t> present, nots, opts;
-            const bool new_group = mode == RG_MODE_SEARCH_PARALLEL || !group_open;
-            if (shape.nested) {
-                // BooleanWeight::create_scorer with groups in this leaf: a group is a DisjunctionSumScorer over its
-                // members present here (even over one: the `1 =>` arm is commented out, boolean_query.rs:196-279),
-                // None when it has none (a required group kills the leaf, an optional one is left out); its cost()
-                // is the sum of those members' doc_freq (disjunction_scorer.rs:39).
-                auto df_of = [&](uint32_t ci) -> uint64_t {
-                    const uint32_t t = clauses[ci].term_id;
-                    return t < seg.host_terms.size() && seg.host_terms[t].doc_freq > 0 ? (uint64_t)seg.host_terms[t].doc_freq : 0;
-                };
-                struct Req { uint64_t cost; QShape::Entry e; std::vector<uint32_t> members; };
-                auto resolve = [&](const QShape::Entry& e, Req& r) {
-                    r = Req{0, e, {}};
-                    if (!e.group) return (r.cost = df_of(e.ci)) > 0;
-                    for (uint32_t j = 0; j < e.n; j++)
-                        if (const uint64_t df = df_of(e.begin + j)) {
-                            r.members.push_back(e.begin + j);
-                            r.cost += df;
-                        }
-                    return !r.members.empty();
-                };
-                std::vector<Req> req, opt;
-                bool dead = false;
-                for (const QShape::Entry& e : shape.req_seq) {
-                    Req r;
-                    if (!resolve(e, r)) dead = true;
-                    req.push_back(std::move(r));
-                }
-                if (dead) continue;
-                for (const QShape::Entry& e : shape.opt_seq) {
-                    Req r;
-                    if (resolve(e, r)) opt.push_back(std::move(r));
-                }
-                for (uint32_t ci : shape.not_idx)
-                    if (df_of(ci)) nots.push_back(ci);
-                std::vector<std::pair<uint64_t, uint32_t>> rreq;
-                std::vector<uint32_t> rnots;
-                if ((!shape.req_rng.empty() || !shape.not_rng.empty()) &&
-                    !resolve_ranges(shape, seg, clauses, ranges, rreq, rnots))
-                    continue;
-                // ConjunctionScorer::new: stable sort by cost() (:30); the score is lead1 + lead2 + the others in
-                // that order, each group one f32 value
-                std::stable_sort(req.begin(), req.end(), [](const Req& a, const Req& b) { return a.cost < b.cost; });
-                // the cheapest required clause leads (a range only when it is cheaper than every term and group)
-                const bool range_lead = !rreq.empty() && (req.empty() || rreq[0].first < req[0].cost);
-                const int leaf_type = shape.type == kTypeReqOpt && opt.empty() ? (int)kTypeAnd : shape.type;
-                const uint64_t cost = range_lead ? rreq[0].first : req[0].cost;
-                uint64_t bytes = 0;
-                for (const Req& r : req) {
-                    if (!r.e.group) bytes += seg.host_terms[clauses[r.e.ci].term_id].enc_bytes;
-                    for (uint32_t ci : r.members) bytes += seg.host_terms[clauses[ci].term_id].enc_bytes;
-                }
-                lp.postings += cost;
-                lp.algo_bytes += bytes + cost;
-                const uint32_t clause_begin = (uint32_t)lp.clauses.size();
-                auto col_of = [&](uint32_t ci) -> int64_t {
-                    if (columns.empty()) return -1;
-                    const rg_clause& c = clauses[ci];
-                    const float w = clause_weight(c);
-                    uint32_t wbits;
-                    memcpy(&wbits, &w, 4);
-                    const auto it = columns.find(ColKey(si, c.term_id, wbits, c.cache_id, k1bits));
-                    return it == columns.end() ? -1 : (int64_t)it->second;
-                };
-                auto range_clause = [&](uint32_t ci, uint32_t not_flag) {
-                    return ItemClause{si * n_ranges + clauses[ci].term_id, 0.0f, 0u, 256u | not_flag};
-                };
-                // a group's members are contiguous, in member order, and always block streams (a group that leads is
-                // merged from its members' blocks); bit9 / bit10: member of a required / optional group, bit11: last
-                auto put = [&](const Req& r, bool lead, uint32_t side) {
-                    if (r.e.group) {
-                        for (size_t j = 0; j < r.members.size(); j++) {
-                            const rg_clause& m = clauses[r.members[j]];
-                            const uint32_t last = j + 1 == r.members.size() ? 2048u : 0u;
-                            lp.clauses.push_back(ItemClause{m.term_id, r.e.filter ? 0.0f : m.weight, m.cache_id,
-                                                            (side == 2u ? 1024u : 512u) | last});
-                        }
-                        return;
-                    }
-                    const rg_clause& c = clauses[r.e.ci];
-                    const float w = side == 2u ? c.weight : clause_weight(c);
-                    const int64_t col = lead ? -1 : col_of(r.e.ci);
-                    if (col >= 0) lp.clauses.push_back(ItemClause{(uint32_t)col, w, c.cache_id, side | 4u});
-                    else lp.clauses.push_back(ItemClause{c.term_id, w, c.cache_id, side});
-                };
-                if (range_lead) lp.clauses.push_back(range_clause(rreq[0].second, 0u));
-                for (size_t i = 0; i < req.size(); i++) put(req[i], i == 0 && !range_lead, 0u);
-                for (size_t i = range_lead ? 1 : 0; i < rreq.size(); i++) lp.clauses.push_back(range_clause(rreq[i].second, 0u));
-                for (uint32_t ci : nots) {
-                    const int64_t col = col_of(ci);
-                    if (col >= 0) lp.clauses.push_back(ItemClause{(uint32_t)col, 0.0f, clauses[ci].cache_id, 1u | 4u});
-                    else lp.clauses.push_back(ItemClause{clauses[ci].term_id, 0.0f, clauses[ci].cache_id, 1u});
-                }
-                for (uint32_t ci : rnots) lp.clauses.push_back(range_clause(ci, 1u));
-                for (const Req& r : opt) put(r, false, 2u);
-                const uint32_t n_item_terms = (uint32_t)(lp.clauses.size() - clause_begin);
-                if (n_item_terms > (uint32_t)kMaxTerms || (!range_lead && req[0].members.size() > 8u))  // a leading group: one warp of k_eval_and_nested per member
-                    throw Unsupported("a nested item wider than k_eval_and_nested takes");  // (n_flat <= 9 keeps this unreachable)
-                // docid ranges as for a conjunction; a ReqOptScorer with a required term or group keeps its running
-                // mean over the whole leaf
-                uint64_t R = std::min<uint64_t>((cost + and_rp - 1) / and_rp, max_ranges);
-                R = std::max<uint64_t>(1, std::min<uint64_t>(R, (uint64_t)(seg.max_doc + kBlock - 1) / kBlock));
-                if (leaf_type == (int)kTypeReqOpt && !req.empty()) R = 1;
-                const uint64_t n_lead_blocks = (uint64_t)(seg.max_doc + kBlock - 1) / kBlock;
+            const uint64_t n_blocks = (uint64_t)(seg.max_doc + kBlock - 1) / kBlock;
+            // The (query, leaf) as R work items, the docid ranges of [0, max_doc) cut evenly (on 128-doc block edges
+            // when a range leads: it walks whole blocks), the next links of the query's heap chain, appended to the
+            // route's launch list; range r gets the launch-order key r * rank_step.
+            auto emit = [&](Route route, uint32_t type, uint32_t n_terms, uint32_t clause_begin, uint32_t width, uint64_t R,
+                            uint32_t rank_step, bool block_edges) {
+                const bool new_group = mode == RG_MODE_SEARCH_PARALLEL || !group_open;
                 if (new_group) {
+                    // SEARCH: one heap per query over all its leaves; SEARCH_PARALLEL: one per leaf
                     lp.group_out.push_back(mode == RG_MODE_SEARCH_PARALLEL ? si * n_queries + qi : qi);
                     group_open = true;
                 }
@@ -1340,70 +1258,155 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
                     WorkItem it{};
                     it.query = qi;
                     it.seg = (uint16_t)si;
-                    it.type = (uint8_t)leaf_type;
-                    it.n_terms = (uint8_t)n_item_terms;
+                    it.type = (uint8_t)type;
+                    it.n_terms = (uint8_t)n_terms;
                     it.lo = (int32_t)((uint64_t)seg.max_doc * r / R);
                     it.hi = (int32_t)((uint64_t)seg.max_doc * (r + 1) / R);
-                    if (range_lead) {
-                        it.lo = (int32_t)(n_lead_blocks * r / R * kBlock);
-                        it.hi = r + 1 == R ? seg.max_doc : (int32_t)(n_lead_blocks * (r + 1) / R * kBlock);
+                    if (block_edges) {
+                        it.lo = (int32_t)(n_blocks * r / R * kBlock);
+                        it.hi = r + 1 == R ? seg.max_doc : (int32_t)(n_blocks * (r + 1) / R * kBlock);
                     }
                     it.clause_begin = clause_begin;
                     it.chain_pos = (r == 0 && new_group) ? 0u : chain_pos;
                     chain_pos = it.chain_pos + 1;
-                    const uint32_t idx = (uint32_t)lp.items.size();
+                    lp.ids[route].push_back((uint32_t)lp.items.size());
+                    if (kRouteByRank[route]) lp.rank[route].push_back((uint32_t)r * rank_step);
                     lp.items.push_back(it);
-                    if (leaf_type == (int)kTypeReqOpt) {
-                        lp.ro_ids.push_back(idx);
-                    } else {
-                        lp.and_ids.push_back(idx);
-                        lp.and_rank.push_back((uint32_t)r);
-                    }
                 }
-                continue;
-            }
-            if (!resolve_leaf(shape, seg, clauses, present, nots, opts)) continue;
-            // point ranges: the required ones with their point counts (cheapest first) and the MUST_NOT ones
-            std::vector<std::pair<uint64_t, uint32_t>> rreq;
-            std::vector<uint32_t> rnots;
-            if ((!shape.req_rng.empty() || !shape.not_rng.empty()) &&
-                !resolve_ranges(shape, seg, clauses, ranges, rreq, rnots))
-                continue;
-            // the cheapest required clause leads: a range's cost is its point count in the leaf, a term's its df
-            const bool range_lead =
-                !rreq.empty() && (present.empty() || rreq[0].first < (uint64_t)seg.host_terms[clauses[present[0]].term_id].doc_freq);
-            auto range_clause = [&](uint32_t ci, uint32_t not_flag) {
-                return ItemClause{si * n_ranges + clauses[ci].term_id, 0.0f, 0u, 256u | not_flag};
+                lp.width[route] = std::max(lp.width[route], width);
             };
-            // no SHOULD scorer in this leaf -> the MUST side alone, no ReqOptScorer (:259-266)
-            // ten or more sub-scorers in this leaf: DisjunctionSumScorer / DisjunctionMaxScorer switch to the
-            // DisiPriorityQueue (disjunction_scorer.rs:41-45,118-139), whose summation order only k_eval_dpq reproduces
-            const bool leaf_dpq = shape.type == kTypeOr && !shape.match_all && present.size() >= 10;
-            const int leaf_type = leaf_dpq ? (int)kTypeDpq
-                                           : (shape.type == kTypeReqOpt && opts.empty() ? (int)kTypeAnd : shape.type);
-            uint64_t cost = 0, bytes = 0, total_df = 0;
-            if (shape.match_all) {
-                cost = total_df = (uint64_t)seg.max_doc;  // AllDocsIterator: every docid of the leaf
-            } else if (range_lead) {
-                cost = total_df = rreq[0].first;
-                bytes = 24ull * ((uint64_t)(seg.max_doc + kBlock - 1) / kBlock) + 8ull * cost;  // block table + keys
-                for (uint32_t ci : present) bytes += seg.host_terms[clauses[ci].term_id].enc_bytes;
-                for (uint32_t ci : opts) bytes += seg.host_terms[clauses[ci].term_id].enc_bytes;
-            } else if (shape.type != kTypeOr) {
-                cost = (uint64_t)seg.host_terms[clauses[present[0]].term_id].doc_freq;
-                const TermHost& lead = seg.host_terms[clauses[present[0]].term_id];
-                bytes = lead.enc_bytes + cost;
-                for (size_t i = 1; i < present.size(); i++) {  // upper bound: min(list, one block per lead doc)
-                    const TermHost& th = seg.host_terms[clauses[present[i]].term_id];
-                    const uint64_t per_block = th.n_blocks ? th.enc_bytes / th.n_blocks : th.enc_bytes;
-                    bytes += std::min<uint64_t>(th.enc_bytes, cost * per_block);
+            auto range_clause = [&](uint32_t ci, uint32_t not_flag) {
+                return ItemClause{si * n_ranges + clauses[ci].term_id, 0.0f, 0u, kClauseRange | not_flag};
+            };
+            const uint32_t clause_begin = (uint32_t)lp.clauses.size();
+            if (shape.type != kTypeOr) {
+                // BooleanWeight::create_scorer of a conjunction / ReqOpt in this leaf.  A term's cost() is its doc_freq.
+                // A group is a DisjunctionSumScorer over its members present here (even over one: the `1 =>` arm is
+                // commented out, boolean_query.rs:196-279), None when it has none; its cost() is the sum of those
+                // members' doc_freq (disjunction_scorer.rs:39).  A required clause that is None leaves the leaf
+                // without a scorer (:201-206), an optional one is left out (:217-234).
+                auto df_of = [&](uint32_t ci) -> uint64_t {
+                    const uint32_t t = clauses[ci].term_id;
+                    return t < seg.host_terms.size() && seg.host_terms[t].doc_freq > 0 ? (uint64_t)seg.host_terms[t].doc_freq : 0;
+                };
+                auto resolve = [&](const QShape::Entry& en) {
+                    Req r{0, (uint32_t)members.size(), 0, en.group, en.filter};
+                    for (uint32_t j = 0; j < en.n; j++)
+                        if (const uint64_t df = df_of(en.begin + j)) {
+                            members.push_back(en.begin + j);
+                            r.cost += df;
+                        }
+                    r.n = (uint32_t)members.size() - r.begin;
+                    return r;
+                };
+                req.clear();
+                opt.clear();
+                members.clear();
+                nots.clear();
+                rreq.clear();
+                rnots.clear();
+                bool dead = shape.req_seq.empty() && shape.req_rng.empty();
+                for (const QShape::Entry& en : shape.req_seq) {
+                    req.push_back(resolve(en));
+                    dead = dead || req.back().n == 0;
                 }
-                for (uint32_t ci : opts) {
+                if (dead) continue;
+                for (const QShape::Entry& en : shape.opt_seq) {
+                    const Req r = resolve(en);
+                    if (r.n) opt.push_back(r);
+                }
+                for (uint32_t ci : shape.not_idx)
+                    if (df_of(ci)) nots.push_back(ci);
+                // point ranges: the required ones with their point counts (cheapest first) and the MUST_NOT ones
+                if ((!shape.req_rng.empty() || !shape.not_rng.empty()) &&
+                    !resolve_ranges(shape, seg, clauses, ranges, rreq, rnots))
+                    continue;
+                // ConjunctionScorer::new: stable sort by cost() (:30); the score is lead1 + lead2 + the others in that
+                // order, each group one f32 value
+                std::stable_sort(req.begin(), req.end(), [](const Req& a, const Req& b) { return a.cost < b.cost; });
+                // the cheapest required clause leads (a range, whose cost is its point count in the leaf, only when it
+                // is cheaper than every term and group)
+                const bool range_lead = !rreq.empty() && (req.empty() || rreq[0].first < req[0].cost);
+                // no SHOULD scorer in this leaf -> the MUST side alone, no ReqOptScorer (:259-266)
+                const uint32_t leaf_type = shape.type == kTypeReqOpt && opt.empty() ? (uint32_t)kTypeAnd : (uint32_t)shape.type;
+                const uint64_t cost = range_lead ? rreq[0].first : req[0].cost;
+                // bytes: the lead's postings (a range lead: its block table and keys, and every clause's list); each
+                // probed term at most one block per lead doc; a group counts as its members
+                auto enc = [&](uint32_t ci) -> uint64_t { return seg.host_terms[clauses[ci].term_id].enc_bytes; };
+                auto probed = [&](uint32_t ci) -> uint64_t {
+                    if (range_lead) return enc(ci);
                     const TermHost& th = seg.host_terms[clauses[ci].term_id];
                     const uint64_t per_block = th.n_blocks ? th.enc_bytes / th.n_blocks : th.enc_bytes;
-                    bytes += std::min<uint64_t>(th.enc_bytes, cost * per_block);
+                    return std::min<uint64_t>(th.enc_bytes, cost * per_block);
+                };
+                uint64_t bytes = range_lead ? 24ull * n_blocks + 8ull * cost : cost;
+                for (size_t i = 0; i < req.size(); i++)
+                    for (uint32_t j = 0; j < req[i].n; j++) {
+                        const uint32_t ci = members[req[i].begin + j];
+                        bytes += i == 0 ? enc(ci) : probed(ci);
+                    }
+                for (const Req& r : opt)
+                    for (uint32_t j = 0; j < r.n; j++) bytes += probed(members[r.begin + j]);
+                for (uint32_t ci : nots) bytes += enc(ci);
+                lp.postings += cost;
+                lp.algo_bytes += bytes;
+                // The lead is a block stream; every other term that has a score column is probed by one gather per
+                // lead doc instead of skip search + block decode (a MUST_NOT term: any column of the term will do).  A
+                // group's members are contiguous, in member order, and always block streams (a group that leads is
+                // merged from its members' blocks).  A range that leads comes first; the other required ranges are
+                // probed after the terms (each adds +0.0f, so where it is added does not change the sum).
+                auto put = [&](const Req& r, bool lead, uint32_t side) {
+                    for (uint32_t j = 0; j < r.n; j++) {
+                        const rg_clause& c = clauses[members[r.begin + j]];
+                        if (r.group) {
+                            const uint32_t last = j + 1 == r.n ? kClauseGroupLast : 0u;
+                            lp.clauses.push_back(ItemClause{c.term_id, r.filter ? 0.0f : c.weight, c.cache_id,
+                                                            (side == kClauseOpt ? kClauseOptGroup : kClauseReqGroup) | last});
+                            continue;
+                        }
+                        const int64_t col = lead ? -1 : col_of(columns, si, c, k1bits);
+                        if (col >= 0) lp.clauses.push_back(ItemClause{(uint32_t)col, clause_weight(c), c.cache_id, side | kClauseColumn});
+                        else lp.clauses.push_back(ItemClause{c.term_id, clause_weight(c), c.cache_id, side});
+                    }
+                };
+                if (range_lead) lp.clauses.push_back(range_clause(rreq[0].second, 0u));
+                for (size_t i = 0; i < req.size(); i++) put(req[i], i == 0 && !range_lead, 0u);
+                for (size_t i = range_lead ? 1 : 0; i < rreq.size(); i++) lp.clauses.push_back(range_clause(rreq[i].second, 0u));
+                for (uint32_t ci : nots) {
+                    const int64_t col = col_of(columns, si, clauses[ci], k1bits);
+                    if (col >= 0) lp.clauses.push_back(ItemClause{(uint32_t)col, 0.0f, clauses[ci].cache_id, kClauseNot | kClauseColumn});
+                    else lp.clauses.push_back(ItemClause{clauses[ci].term_id, 0.0f, clauses[ci].cache_id, kClauseNot});
                 }
-                total_df = cost;
+                for (uint32_t ci : rnots) lp.clauses.push_back(range_clause(ci, kClauseNot));
+                for (const Req& r : opt) put(r, false, kClauseOpt);
+                const uint32_t n_item_terms = (uint32_t)(lp.clauses.size() - clause_begin);
+                if (n_item_terms > (uint32_t)kMaxTerms || (!range_lead && req[0].group && req[0].n > 8u))  // a leading group: one warp of k_eval_and_nested per member
+                    throw Unsupported("a conjunction item wider than k_eval_and takes");  // (the classifiers keep this unreachable)
+                // Ranges of ~range_postings postings, at most max_ranges per (query, leaf).  A ReqOptScorer with a
+                // required term or group keeps its running mean over the whole leaf: one item.  One whose required
+                // side is only ranges scores +0.0f there, so scores_sum stays 0, 2 * 0 < 0 never holds and the running
+                // mean never skips the optional side: its docid ranges are independent.
+                uint64_t R = std::min<uint64_t>((cost + and_rp - 1) / and_rp, max_ranges);
+                R = std::max<uint64_t>(1, std::min<uint64_t>(R, n_blocks));
+                if (leaf_type == kTypeReqOpt && !req.empty()) R = 1;
+                bool grouped = false;
+                for (const Req& r : req) grouped = grouped || r.group;
+                for (const Req& r : opt) grouped = grouped || r.group;
+                const bool ro = leaf_type == kTypeReqOpt;
+                const Route route = grouped                             ? (ro ? kRouteReqOptNested : kRouteAndNested)
+                                    : !rreq.empty() || !rnots.empty() ? (ro ? kRouteReqOptRanges : kRouteAndRanges)
+                                                                      : (ro ? kRouteReqOpt : kRouteAnd);
+                emit(route, leaf_type, n_item_terms, clause_begin, 0u, R, 1u, range_lead);
+                continue;
+            }
+            // disjunctions: present = the scoring clauses, nots = the MUST_NOT ones
+            if (!resolve_leaf(shape, seg, clauses, present, nots, opts)) continue;
+            // ten or more sub-scorers in this leaf: DisjunctionSumScorer / DisjunctionMaxScorer switch to the
+            // DisiPriorityQueue (disjunction_scorer.rs:41-45,118-139), whose summation order only k_eval_dpq reproduces
+            const bool leaf_dpq = !shape.match_all && present.size() >= 10;
+            uint64_t cost = 0, bytes = 0;
+            if (shape.match_all) {
+                cost = (uint64_t)seg.max_doc;  // AllDocsIterator: every docid of the leaf
             } else {
                 for (uint32_t ci : present) {
                     const TermHost& th = seg.host_terms[clauses[ci].term_id];
@@ -1411,22 +1414,10 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
                     bytes += th.enc_bytes + 12ull * th.n_blocks;  // + skip table / descriptors
                 }
                 bytes += cost;  // one norm byte per scored posting
-                total_df = cost;
             }
             for (uint32_t ci : nots) bytes += seg.host_terms[clauses[ci].term_id].enc_bytes;
-            lp.postings += total_df;
+            lp.postings += cost;
             lp.algo_bytes += bytes;
-            const uint32_t clause_begin = (uint32_t)lp.clauses.size();
-            // score column of a clause in this leaf (-1: none)
-            auto col_of = [&](uint32_t ci) -> int64_t {
-                if (columns.empty()) return -1;
-                const rg_clause& c = clauses[ci];
-                const float w = clause_weight(c);
-                uint32_t wbits;
-                memcpy(&wbits, &w, 4);
-                const auto it = columns.find(ColKey(si, c.term_id, wbits, c.cache_id, k1bits));
-                return it == columns.end() ? -1 : (int64_t)it->second;
-            };
             auto df_of = [&](uint32_t ci) { return (uint64_t)seg.host_terms[clauses[ci].term_id].doc_freq; };
             bool use_ms = false;
             uint32_t n_streams = 0;
@@ -1436,10 +1427,10 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
                 // the leaf's match-all column (every docid present, score 0) + the MUST_NOT streams: k_eval_or<NOT>
                 const auto it = columns.find(ColKey(si, kMatchAllTerm, 0u, 0u, 0u));
                 if (it == columns.end()) throw Unsupported("no memory for the MatchAllDocsQuery column");
-                lp.clauses.push_back(ItemClause{it->second, 0.0f, 0u, 4u | 16u | 64u});  // 64: every docid present
+                lp.clauses.push_back(ItemClause{it->second, 0.0f, 0u, kClauseColumn | kClauseNoBound | kClauseAllDocs});
             } else if (leaf_dpq) {
                 for (uint32_t ci : present) lp.clauses.push_back(ItemClause{clauses[ci].term_id, clause_weight(clauses[ci]), clauses[ci].cache_id, 0});
-            } else if (shape.type == kTypeOr) {
+            } else {
                 // A disjunction goes to k_eval_or_ms (presence bitmaps, non-essential clauses are only counted)
                 // when it is a plain sum of SHOULD clauses, reads at least one score column, and none of its
                 // other clauses is dense (a dense block stream would cut its windows to a few docids).
@@ -1452,23 +1443,22 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
                 use_ms = !no_ms && n_bitmap > 0 && !dense_stream && nots.empty() && !shape.msm && !(shape.dismax && present.size() > 1);
                 for (uint32_t ci : present) {
                     const rg_clause& c = clauses[ci];
-                    const int64_t col = col_of(ci);
+                    const int64_t col = col_of(columns, si, c, k1bits);
                     const float w = clause_weight(c);
-                    // bit4: the score bound w*(k1+1) needs weight >= 0 and cache entries >= 0
+                    // the score bound w*(k1+1) needs weight >= 0 and cache entries >= 0
                     const bool boundable = w >= 0.0f && w < INFINITY && k1 >= 0.0f &&
                                            c.cache_id < e->cache_nonneg.size() && e->cache_nonneg[c.cache_id];
+                    const uint32_t bound = boundable ? 0u : kClauseNoBound;
                     // the exhaustive kernel scans a column docid by docid: that only pays for df >= max_doc/8
                     if (col >= 0 && (use_ms || df_of(ci) * e->or_col_den >= (uint64_t)seg.max_doc)) {
-                        lp.clauses.push_back(ItemClause{(uint32_t)col, w, c.cache_id, 4u | (boundable ? 0u : 16u)});
+                        lp.clauses.push_back(ItemClause{(uint32_t)col, w, c.cache_id, kClauseColumn | bound});
                         continue;
                     }
                     n_streams++;
                     uint32_t flags = 0;
                     if (!use_ms && !lists.empty()) {  // a scored list of this clause: streamed instead of decoded
-                        uint32_t wbits;
-                        memcpy(&wbits, &w, 4);
-                        const auto lt = lists.find(ColKey(si, c.term_id, wbits, c.cache_id, k1bits));
-                        if (lt != lists.end()) flags = 128u | (lt->second << 16);
+                        const auto lt = lists.find(col_key(si, c, k1bits));
+                        if (lt != lists.end()) flags = kClauseList | (lt->second << kClauseRefShift);
                     }
                     if (use_ms && seg.bitmap_slot[c.term_id] >= 0) {  // a block stream whose presence comes from its bitmap
                         const auto key = std::make_tuple(si, c.term_id, c.cache_id);
@@ -1481,110 +1471,43 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
                             tf_planes_of(e, si, c.term_id, c.cache_id, k1, ref);
                             hp.col_refs.push_back(ref);
                         }
-                        if (it->second < 65536u) flags = 32u | (boundable ? 0u : 16u) | (it->second << 16);
+                        if (it->second < 65536u) flags = kClauseBitmap | bound | (it->second << kClauseRefShift);
                     }
                     lp.clauses.push_back(ItemClause{c.term_id, w, c.cache_id, flags});
                 }
-            } else {
-                // conjunction: the lead (cheapest) clause is a block stream; every other clause that has a score
-                // column is probed by one gather per lead doc instead of skip search + block decode
-                // a range that leads comes first; the other required ranges are probed after the terms (each adds
-                // +0.0f, so where it is added does not change the sum)
-                if (range_lead) lp.clauses.push_back(range_clause(rreq[0].second, 0u));
-                for (size_t i = 0; i < present.size(); i++) {
-                    const rg_clause& c = clauses[present[i]];
-                    const int64_t col = (i == 0 && !range_lead) ? -1 : col_of(present[i]);
-                    if (col >= 0) lp.clauses.push_back(ItemClause{(uint32_t)col, clause_weight(c), c.cache_id, 4u});
-                    else lp.clauses.push_back(ItemClause{c.term_id, clause_weight(c), c.cache_id, 0});
-                }
-                for (size_t i = range_lead ? 1 : 0; i < rreq.size(); i++) lp.clauses.push_back(range_clause(rreq[i].second, 0u));
             }
-            for (uint32_t ci : nots) {
-                const int64_t col = shape.type == kTypeOr ? -1 : col_of(ci);  // conjunctions: any column of the term will do
-                if (col >= 0) lp.clauses.push_back(ItemClause{(uint32_t)col, 0.0f, clauses[ci].cache_id, 1u | 4u});
-                else lp.clauses.push_back(ItemClause{clauses[ci].term_id, 0.0f, clauses[ci].cache_id, 1u});
-            }
-            for (uint32_t ci : rnots) lp.clauses.push_back(range_clause(ci, 1u));
-            for (uint32_t ci : opts) {
-                const int64_t col = col_of(ci);
-                if (col >= 0) lp.clauses.push_back(ItemClause{(uint32_t)col, clauses[ci].weight, clauses[ci].cache_id, 2u | 4u});
-                else lp.clauses.push_back(ItemClause{clauses[ci].term_id, clauses[ci].weight, clauses[ci].cache_id, 2u});
-            }
-            const uint32_t n_item_terms =
-                (uint32_t)(present.size() + (shape.match_all ? 1 : 0) + nots.size() + opts.size() + rreq.size() + rnots.size());
+            for (uint32_t ci : nots) lp.clauses.push_back(ItemClause{clauses[ci].term_id, 0.0f, clauses[ci].cache_id, kClauseNot});
+            const uint32_t n_item_terms = (uint32_t)(present.size() + (shape.match_all ? 1 : 0) + nots.size());
             // DisjunctionMaxWeight::create_scorer (disjunction_max_query.rs:135-155): one scorer in this
             // leaf is that scorer; otherwise the tie breaker rides in a meta clause after the item's
             const bool leaf_dismax = shape.dismax && present.size() > 1;
             // the decode-free k_eval_or: a plain sum whose every clause is a score column or a scored list
-            bool lean = lists_on && leaf_type == (int)kTypeOr && !use_ms && item_pos && nots.empty() && !shape.msm && !leaf_dismax;
-            for (uint32_t i = clause_begin; lean && i < lp.clauses.size(); i++) lean = (lp.clauses[i].flags & (4u | 128u)) != 0;
-            if (leaf_dismax) lp.clauses.push_back(ItemClause{0u, shape.tie, 0u, 8u});
+            bool lean = lists_on && !leaf_dpq && !use_ms && item_pos && nots.empty() && !shape.msm && !leaf_dismax;
+            for (uint32_t i = clause_begin; lean && i < lp.clauses.size(); i++)
+                lean = (lp.clauses[i].flags & (kClauseColumn | kClauseList)) != 0;
+            if (leaf_dismax) lp.clauses.push_back(ItemClause{0u, shape.tie, 0u, kClauseTie});
             // ranges of ~range_postings postings, at most max_ranges per (query, leaf): long lists get
             // longer ranges (a range is one warp's sequential job; there are thousands of warps)
-            const uint64_t range_postings = leaf_type == (int)kTypeOr ? or_rp : and_rp;
-            uint64_t R = (cost + range_postings - 1) / range_postings;
-            R = std::min<uint64_t>(R, max_ranges);
+            uint64_t R = std::min<uint64_t>((cost + or_rp - 1) / or_rp, max_ranges);
             uint32_t rank_step = 1;  // launch-order key of range r = r * rank_step (its start on the leaf's grid)
-            if (leaf_type == (int)kTypeOr && or_grid[si]) {
+            if (or_grid[si]) {
                 R = or_grid[si];
                 while (R > 1 && cost / R < (1u << 13)) {
                     R >>= 1;
                     rank_step <<= 1;
                 }
             }
-            R = std::max<uint64_t>(1, std::min<uint64_t>(R, (uint64_t)(seg.max_doc + kBlock - 1) / kBlock));
-            // sequential scorer state: one item per leaf.  Except a ReqOptScorer whose required side is only ranges:
-            // its required score is +0.0f, so scores_sum stays 0, 2 * 0 < 0 never holds and the running mean never
-            // skips the optional side — the docid ranges are independent
-            if ((leaf_type == (int)kTypeReqOpt && !present.empty()) || leaf_dpq) R = 1;
-            const uint64_t n_lead_blocks = (uint64_t)(seg.max_doc + kBlock - 1) / kBlock;
-            if (new_group) {
-                // SEARCH: one heap per query over all its leaves; SEARCH_PARALLEL: one per leaf
-                lp.group_out.push_back(mode == RG_MODE_SEARCH_PARALLEL ? si * n_queries + qi : qi);
-                group_open = true;
+            R = std::max<uint64_t>(1, std::min<uint64_t>(R, n_blocks));
+            if (leaf_dpq) R = 1;  // sequential scorer state: one item per leaf
+            const Route route = leaf_dpq ? kRouteDpq : use_ms ? kRouteMs : lean ? kRouteLean : kRouteOr;
+            if (route == kRouteOr) {  // the k_eval_or variant the batch needs
+                lp.or_has_not = lp.or_has_not || !nots.empty();
+                lp.or_nonpos = lp.or_nonpos || !item_pos;
+                lp.or_has_msm = lp.or_has_msm || shape.msm;
+                lp.or_has_dmax = lp.or_has_dmax || leaf_dismax;
             }
-            for (uint64_t r = 0; r < R; r++) {
-                WorkItem it{};
-                it.query = qi;
-                it.seg = (uint16_t)si;
-                it.type = (uint8_t)(leaf_type | (shape.type == kTypeOr ? shape.msm << 4 : 0u) | (leaf_dismax ? 4u : 0u));
-                it.n_terms = (uint8_t)n_item_terms;
-                it.lo = (int32_t)((uint64_t)seg.max_doc * r / R);
-                it.hi = (int32_t)((uint64_t)seg.max_doc * (r + 1) / R);
-                if (range_lead) {  // a range lead walks whole 128-doc blocks: cut on block edges
-                    it.lo = (int32_t)(n_lead_blocks * r / R * kBlock);
-                    it.hi = r + 1 == R ? seg.max_doc : (int32_t)(n_lead_blocks * (r + 1) / R * kBlock);
-                }
-                it.clause_begin = clause_begin;
-                it.chain_pos = (r == 0 && new_group) ? 0u : chain_pos;
-                chain_pos = it.chain_pos + 1;
-                const uint32_t idx = (uint32_t)lp.items.size();
-                lp.items.push_back(it);
-                if (leaf_dpq) {
-                    lp.dpq_ids.push_back(idx);
-                    lp.max_dpq_terms = std::max<uint32_t>(lp.max_dpq_terms, n_item_terms);
-                } else if (leaf_type == (int)kTypeReqOpt) {
-                    lp.ro_ids.push_back(idx);
-                } else if (leaf_type == (int)kTypeAnd) {
-                    lp.and_ids.push_back(idx);
-                    lp.and_rank.push_back((uint32_t)r);
-                } else if (use_ms) {
-                    lp.ms_ids.push_back(idx);
-                    lp.ms_rank.push_back((uint32_t)r * rank_step);
-                    lp.max_ms_streams = std::max<uint32_t>(lp.max_ms_streams, n_streams);
-                } else if (lean) {
-                    lp.lean_ids.push_back(idx);
-                    lp.lean_rank.push_back((uint32_t)r * rank_step);
-                } else {
-                    lp.or_ids.push_back(idx);
-                    lp.or_rank.push_back((uint32_t)r * rank_step);
-                    lp.max_or_terms = std::max<uint32_t>(lp.max_or_terms, n_item_terms);
-                    if (!nots.empty()) lp.or_has_not = true;
-                    if (!item_pos) lp.or_nonpos = true;
-                    if (shape.msm) lp.or_has_msm = true;
-                    if (leaf_dismax) lp.or_has_dmax = true;
-                }
-            }
+            const uint32_t type = (leaf_dpq ? kTypeDpq : kTypeOr) | shape.msm << kItemMsmShift | (leaf_dismax ? kItemDismax : 0u);
+            emit(route, type, n_item_terms, clause_begin, route == kRouteMs ? n_streams : n_item_terms, R, rank_step, false);
         }
     }
     };
@@ -1610,18 +1533,19 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
         for (auto& ep : errs)
             if (ep) std::rethrow_exception(ep);
         // concatenate in query order: offsets first, then every part is copied by its own thread
-        struct Off { size_t items, clauses, or_ids, ms_ids, and_ids, ro_ids, dpq_ids, lean_ids, groups; };
-        std::vector<Off> off(n_threads + 1, Off{0, 0, 0, 0, 0, 0, 0, 0, 0});
+        struct Off { size_t items, clauses, groups, ids[kRoutes]; };
+        std::vector<Off> off(n_threads + 1, Off{});
         for (uint32_t t = 0; t < n_threads; t++) {
             const HostPlan& lp = parts[t];
-            off[t + 1] = Off{off[t].items + lp.items.size(), off[t].clauses + lp.clauses.size(), off[t].or_ids + lp.or_ids.size(),
-                             off[t].ms_ids + lp.ms_ids.size(), off[t].and_ids + lp.and_ids.size(), off[t].ro_ids + lp.ro_ids.size(),
-                             off[t].dpq_ids + lp.dpq_ids.size(), off[t].lean_ids + lp.lean_ids.size(), off[t].groups + lp.group_out.size()};
+            off[t + 1].items = off[t].items + lp.items.size();
+            off[t + 1].clauses = off[t].clauses + lp.clauses.size();
+            off[t + 1].groups = off[t].groups + lp.group_out.size();
+            for (uint32_t r = 0; r < kRoutes; r++) {
+                off[t + 1].ids[r] = off[t].ids[r] + lp.ids[r].size();
+                hp.width[r] = std::max(hp.width[r], lp.width[r]);
+            }
             hp.postings += lp.postings;
             hp.algo_bytes += lp.algo_bytes;
-            hp.max_or_terms = std::max(hp.max_or_terms, lp.max_or_terms);
-            hp.max_ms_streams = std::max(hp.max_ms_streams, lp.max_ms_streams);
-            hp.max_dpq_terms = std::max(hp.max_dpq_terms, lp.max_dpq_terms);
             hp.or_has_not = hp.or_has_not || lp.or_has_not;
             hp.or_nonpos = hp.or_nonpos || lp.or_nonpos;
             hp.or_has_msm = hp.or_has_msm || lp.or_has_msm;
@@ -1630,17 +1554,11 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
         const Off& end = off[n_threads];
         hp.items.resize(end.items);
         hp.clauses.resize(end.clauses);
-        hp.or_ids.resize(end.or_ids);
-        hp.or_rank.resize(end.or_ids);
-        hp.ms_ids.resize(end.ms_ids);
-        hp.ms_rank.resize(end.ms_ids);
-        hp.and_ids.resize(end.and_ids);
-        hp.and_rank.resize(end.and_ids);
-        hp.ro_ids.resize(end.ro_ids);
-        hp.dpq_ids.resize(end.dpq_ids);
-        hp.lean_ids.resize(end.lean_ids);
-        hp.lean_rank.resize(end.lean_ids);
         hp.group_out.resize(end.groups);
+        for (uint32_t r = 0; r < kRoutes; r++) {
+            hp.ids[r].resize(end.ids[r]);
+            if (kRouteByRank[r]) hp.rank[r].resize(end.ids[r]);
+        }
         ths.clear();
         for (uint32_t t = 0; t < n_threads; t++)
             ths.emplace_back([&, t] {
@@ -1653,19 +1571,10 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
                     hp.items[o.items + i] = it;
                 }
                 std::copy(lp.clauses.begin(), lp.clauses.end(), hp.clauses.begin() + o.clauses);
-                auto put_ids = [&](std::vector<uint32_t>& dst, size_t at, const std::vector<uint32_t>& src) {
-                    for (size_t i = 0; i < src.size(); i++) dst[at + i] = src[i] + item_off;
-                };
-                put_ids(hp.or_ids, o.or_ids, lp.or_ids);
-                put_ids(hp.ms_ids, o.ms_ids, lp.ms_ids);
-                put_ids(hp.and_ids, o.and_ids, lp.and_ids);
-                put_ids(hp.ro_ids, o.ro_ids, lp.ro_ids);
-                put_ids(hp.dpq_ids, o.dpq_ids, lp.dpq_ids);
-                put_ids(hp.lean_ids, o.lean_ids, lp.lean_ids);
-                std::copy(lp.lean_rank.begin(), lp.lean_rank.end(), hp.lean_rank.begin() + o.lean_ids);
-                std::copy(lp.or_rank.begin(), lp.or_rank.end(), hp.or_rank.begin() + o.or_ids);
-                std::copy(lp.ms_rank.begin(), lp.ms_rank.end(), hp.ms_rank.begin() + o.ms_ids);
-                std::copy(lp.and_rank.begin(), lp.and_rank.end(), hp.and_rank.begin() + o.and_ids);
+                for (uint32_t r = 0; r < kRoutes; r++) {
+                    for (size_t i = 0; i < lp.ids[r].size(); i++) hp.ids[r][o.ids[r] + i] = lp.ids[r][i] + item_off;
+                    std::copy(lp.rank[r].begin(), lp.rank[r].end(), hp.rank[r].begin() + o.ids[r]);
+                }
                 std::copy(lp.group_out.begin(), lp.group_out.end(), hp.group_out.begin() + o.groups);
             });
         for (auto& th : ths) th.join();
@@ -1686,28 +1595,8 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
         for (size_t i = 0; i < ids.size(); i++) out[start[rank[i]]++] = ids[i];
         ids.swap(out);
     };
-    by_rank(hp.or_ids, hp.or_rank);
-    by_rank(hp.ms_ids, hp.ms_rank);
-    by_rank(hp.lean_ids, hp.lean_rank);
-    by_rank(hp.and_ids, hp.and_rank);
-    auto split = [&](std::vector<uint32_t>& ids, std::vector<uint32_t>& out_ids, uint32_t flags) {
-        std::vector<uint32_t> keep;
-        for (uint32_t id : ids) {
-            const WorkItem& it = hp.items[id];
-            bool r = false;
-            for (uint32_t c = 0; c < it.n_terms; c++) r = r || (hp.clauses[it.clause_begin + c].flags & flags) != 0;
-            (r ? out_ids : keep).push_back(id);
-        }
-        ids.swap(keep);
-    };
-    if (any_groups) {  // items with a group go to k_eval_and_nested (ranges or not), in the same launch order
-        split(hp.and_ids, hp.and_grp_ids, 512u | 1024u);
-        split(hp.ro_ids, hp.ro_grp_ids, 512u | 1024u);
-    }
-    if (any_ranges) {  // items with a range clause go to k_eval_and_ranges, in the same launch order
-        split(hp.and_ids, hp.and_rng_ids, 256u);
-        split(hp.ro_ids, hp.ro_rng_ids, 256u);
-    }
+    for (uint32_t r = 0; r < kRoutes; r++)
+        if (kRouteByRank[r]) by_rank(hp.ids[r], hp.rank[r]);
     // heap groups = contiguous item runs starting at chain-start items
     for (uint32_t i = 0; i < hp.items.size(); i++)
         if (hp.items[i].chain_pos == 0) hp.group_item_begin.push_back(i);
@@ -1741,9 +1630,7 @@ void plan_rescore(const rg_engine* e, const rg_query* queries, uint32_t n_querie
         // DisjunctionSumScorer over whatever SHOULD clauses exist in the leaf, however few: min_should_match plays
         // no part in rescoring
         shape.msm = 0;
-        for (const auto* idx : {&shape.clause_idx, &shape.opt_idx, &shape.not_idx})
-            for (uint32_t ci : *idx)
-                if (clauses[ci].cache_id >= n_caches) throw ArgError("clause refers to an unset norm cache");
+        check_caches(shape, clauses, n_caches);
         // a bare TermQuery, or what BooleanQuery::build / DisjunctionMaxQuery::build collapse to one clause: the
         // TermScorer itself (a DisjunctionSumScorer would add it to 0.0f)
         const bool single = shape.type == kTypeOr && !shape.match_all && !shape.dismax && shape.clause_idx.size() == 1 &&
@@ -1844,7 +1731,7 @@ static std::vector<uint2> deep_bucket_maps(const rg_engine* e, const HostPlan& h
         float u = 0.0f;
         for (uint32_t c = 0; c < it.n_terms; c++) {
             const ItemClause& ic = hp.clauses[it.clause_begin + c];
-            if (ic.flags & (1u | 8u | 64u | 256u)) continue;
+            if (ic.flags & (kClauseNot | kClauseTie | kClauseAllDocs | kClauseRange)) continue;
             const float w1 = ic.weight * (k1 + 1.0f);
             if (w1 == 0.0f) continue;  // scores +-0 only (FILTER): an all-zero query keeps the absolute map, whose edge 128 is +0
             const bool nonneg = ic.cache_id < e->cache_nonneg.size() && e->cache_nonneg[ic.cache_id];
@@ -1868,6 +1755,22 @@ static std::vector<uint2> deep_bucket_maps(const rg_engine* e, const HostPlan& h
         }
     }
     return maps;
+}
+
+// The range / group array of a *_ranges / *_nested entry point: NULL with a non-zero count is a null argument;
+// otherwise a non-null array (even of length 0) makes the range / group clauses readable.
+template <class T>
+bool readable(const T*& a, uint32_t n) {
+    static const T none{};
+    if (n && !a) return false;
+    if (!a) a = &none;
+    return true;
+}
+
+int null_argument(rg_batch** out) {
+    if (out) *out = nullptr;
+    g_last_error = "null argument";
+    return RG_EINVAL;
 }
 
 }  // namespace
@@ -1908,26 +1811,17 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
     b->n_lists_built = hp.n_lists_built;
     b->list_floats = hp.list_floats;
     b->col_floats = hp.col_floats;
-    b->n_ms = (uint32_t)hp.ms_ids.size();
-    b->n_lean = (uint32_t)hp.lean_ids.size();
-    b->max_ms_streams = hp.max_ms_streams;
     for (const ColRef& r : hp.col_refs) b->uses_planes = b->uses_planes || r.hi1 != nullptr;
-    b->n_dpq = (uint32_t)hp.dpq_ids.size();
-    b->max_dpq_terms = hp.max_dpq_terms;
     b->n_queries = n_queries;
     b->k = p->k;
     b->mode = p->mode;
     b->k1 = p->k1;
     b->n_items = (uint32_t)hp.items.size();
-    b->n_or = (uint32_t)hp.or_ids.size();
-    b->n_and = (uint32_t)hp.and_ids.size();
-    b->n_ro = (uint32_t)hp.ro_ids.size();
-    b->n_and_rng = (uint32_t)hp.and_rng_ids.size();
-    b->n_ro_rng = (uint32_t)hp.ro_rng_ids.size();
-    b->n_and_grp = (uint32_t)hp.and_grp_ids.size();
-    b->n_ro_grp = (uint32_t)hp.ro_grp_ids.size();
+    for (uint32_t r = 0; r < kRoutes; r++) {
+        b->n_ids[r] = (uint32_t)hp.ids[r].size();
+        b->width[r] = hp.width[r];
+    }
     b->n_groups = (uint32_t)hp.group_out.size();
-    b->max_or_terms = hp.max_or_terms;
     b->or_has_not = hp.or_has_not;
     b->or_nonpos = hp.or_nonpos;
     b->or_has_msm = hp.or_has_msm;
@@ -1950,21 +1844,12 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
     };
     carve(b->items, hp.items.size());
     carve(b->clauses, hp.clauses.size());
-    carve(b->or_ids, hp.or_ids.size());
-    carve(b->and_ids, hp.and_ids.size());
-    carve(b->ms_ids, hp.ms_ids.size());
-    carve(b->dpq_ids, hp.dpq_ids.size());
-    carve(b->ro_ids, hp.ro_ids.size());
+    for (uint32_t r = 0; r < kRoutes; r++) carve(b->ids[r], hp.ids[r].size());
     carve(b->col_refs, hp.col_refs.size());
-    carve(b->lean_ids, hp.lean_ids.size());
     carve(b->local_lists, hp.local_floats / 4);
     carve(b->group_item_begin, hp.group_item_begin.size());
     carve(b->group_out, hp.group_out.size());
     carve(b->range_refs, hp.range_refs.size());
-    carve(b->and_rng_ids, hp.and_rng_ids.size());
-    carve(b->ro_rng_ids, hp.ro_rng_ids.size());
-    carve(b->and_grp_ids, hp.and_grp_ids.size());
-    carve(b->ro_grp_ids, hp.ro_grp_ids.size());
     // running top-k scores of every OR work item (theta inheritance along a heap chain); skipped when it would
     // not fit comfortably (huge batches with k near 1024): theta then falls back to the per-range bound.  Deep
     // batches keep a score histogram of every item there instead (1 KB each)
@@ -2008,13 +1893,12 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
         using T = std::remove_reference_t<decltype(*span.p)>;
         span.p = reinterpret_cast<T*>(b->slab.p + reinterpret_cast<size_t>(span.p));
     };
-    rebase(b->items); rebase(b->clauses); rebase(b->or_ids); rebase(b->and_ids); rebase(b->ms_ids); rebase(b->dpq_ids); rebase(b->ro_ids); rebase(b->col_refs);
-    rebase(b->lean_ids); rebase(b->local_lists);
+    rebase(b->items); rebase(b->clauses); rebase(b->col_refs); rebase(b->local_lists);
+    for (Span<uint32_t>& ids : b->ids) rebase(ids);
     rebase(b->group_item_begin); rebase(b->group_out); rebase(b->item_head); rebase(b->item_matches);
     rebase(b->item_theta); rebase(b->item_topk_n); rebase(b->item_topk); rebase(b->arena_next); rebase(b->dbg); rebase(b->out_hits); rebase(b->out_counts);
     rebase(b->out_total);
-    rebase(b->range_refs); rebase(b->and_rng_ids); rebase(b->ro_rng_ids); rebase(b->range_stats);
-    rebase(b->and_grp_ids); rebase(b->ro_grp_ids); rebase(b->group_stats);
+    rebase(b->range_refs); rebase(b->range_stats); rebase(b->group_stats);
     if (p->mode == RG_MODE_SEARCH_PARALLEL) rebase(b->leaf_records);
     if (deep) rebase(b->deep_map);
     b->zero_begin = b->slab.p + zero_off;
@@ -2024,20 +1908,11 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
     cudaStream_t cs = e->copy_stream;
     up(b->items, hp.items, cs);
     up(b->clauses, hp.clauses, cs);
-    up(b->or_ids, hp.or_ids, cs);
-    up(b->and_ids, hp.and_ids, cs);
-    up(b->ms_ids, hp.ms_ids, cs);
-    up(b->dpq_ids, hp.dpq_ids, cs);
-    up(b->ro_ids, hp.ro_ids, cs);
-    up(b->lean_ids, hp.lean_ids, cs);
+    for (uint32_t r = 0; r < kRoutes; r++) up(b->ids[r], hp.ids[r], cs);
     up(b->col_refs, hp.col_refs, cs);
     up(b->group_item_begin, hp.group_item_begin, cs);
     up(b->group_out, hp.group_out, cs);
     up(b->range_refs, hp.range_refs, cs);
-    up(b->and_rng_ids, hp.and_rng_ids, cs);
-    up(b->ro_rng_ids, hp.ro_rng_ids, cs);
-    up(b->and_grp_ids, hp.and_grp_ids, cs);
-    up(b->ro_grp_ids, hp.ro_grp_ids, cs);
     if (deep) up(b->deep_map, deep_maps, cs);
     RG_CUDA_CHECK(cudaEventCreateWithFlags(&b->uploaded, cudaEventDisableTiming));
     RG_CUDA_CHECK(cudaEventCreateWithFlags(&b->done, cudaEventDisableTiming));
@@ -2058,12 +1933,13 @@ static int batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queri
         tm.mark("local_lists_build");
     }
     b->h2d_bytes = (hp.items.size() * sizeof(WorkItem)) + hp.clauses.size() * sizeof(ItemClause) +
-                   4 * (hp.or_ids.size() + hp.lean_ids.size() + hp.ms_ids.size() + hp.dpq_ids.size() + hp.and_ids.size() + hp.ro_ids.size() + hp.group_item_begin.size() + hp.group_out.size()) +
-                   hp.col_refs.size() * sizeof(ColRef) + hp.range_refs.size() * sizeof(RangeRef) +
-                   4 * (hp.and_rng_ids.size() + hp.ro_rng_ids.size() + hp.and_grp_ids.size() + hp.ro_grp_ids.size());
-    b->kernels_per_run = (b->n_lean ? 1 : 0) + (b->n_ms ? 1 : 0) + (b->n_dpq ? 1 : 0) + (b->n_or ? 1 : 0) + (b->n_and ? 1 : 0) + (b->n_ro ? 1 : 0) + (b->n_groups ? 1 : 0) +
-                         (p->mode == RG_MODE_SEARCH_PARALLEL ? 1 : 0) + (b->n_and_rng ? 1 : 0) + (b->n_ro_rng ? 1 : 0) +
-                         (b->n_and_grp ? 1 : 0) + (b->n_ro_grp ? 1 : 0);
+                   4 * (hp.group_item_begin.size() + hp.group_out.size()) + hp.col_refs.size() * sizeof(ColRef) +
+                   hp.range_refs.size() * sizeof(RangeRef);
+    b->kernels_per_run = (b->n_groups ? 1 : 0) + (p->mode == RG_MODE_SEARCH_PARALLEL ? 1 : 0);
+    for (uint32_t r = 0; r < kRoutes; r++) {
+        b->h2d_bytes += 4 * hp.ids[r].size();
+        b->kernels_per_run += b->n_ids[r] ? 1 : 0;
+    }
     tm.mark("alloc_copy_issue");
     RG_CUDA_CHECK(cudaStreamSynchronize(cs));  // the host vectors go out of scope (a running batch is not waited for)
     tm.mark("sync");
@@ -2081,29 +1957,15 @@ int rg_batch_prepare(rg_engine* e, const rg_query* queries, uint32_t n_queries,
 int rg_batch_prepare_ranges(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
                             uint32_t n_clauses, const rg_search_params* p, const rg_point_range* ranges,
                             uint32_t n_ranges, rg_batch** out) {
-    if (n_ranges && !ranges) {
-        if (out) *out = nullptr;
-        g_last_error = "null argument";
-        return RG_EINVAL;
-    }
-    // a non-null array (even of length 0) makes range clauses readable
-    static const rg_point_range none{};
-    return batch_prepare(e, queries, n_queries, clauses, n_clauses, p, ranges ? ranges : &none, n_ranges, out);
+    if (!readable(ranges, n_ranges)) return null_argument(out);
+    return batch_prepare(e, queries, n_queries, clauses, n_clauses, p, ranges, n_ranges, out);
 }
 
 int rg_batch_prepare_nested(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
                             uint32_t n_clauses, const rg_search_params* p, const rg_point_range* ranges,
                             uint32_t n_ranges, const rg_query* groups, uint32_t n_groups, rg_batch** out) {
-    if ((n_ranges && !ranges) || (n_groups && !groups)) {
-        if (out) *out = nullptr;
-        g_last_error = "null argument";
-        return RG_EINVAL;
-    }
-    // non-null arrays (even of length 0) make range and group clauses readable
-    static const rg_point_range none{};
-    static const rg_query no_group{};
-    return batch_prepare(e, queries, n_queries, clauses, n_clauses, p, ranges ? ranges : &none, n_ranges, out,
-                         groups ? groups : &no_group, n_groups);
+    if (!readable(ranges, n_ranges) || !readable(groups, n_groups)) return null_argument(out);
+    return batch_prepare(e, queries, n_queries, clauses, n_clauses, p, ranges, n_ranges, out, groups, n_groups);
 }
 
 int rg_batch_run(rg_engine* e, rg_batch* b) {
@@ -2144,27 +2006,27 @@ int rg_batch_run(rg_engine* e, rg_batch* b) {
         has_live = has_live || sg.live.p != nullptr;
         has_other = has_other || sg.has_other_enc;
     }
-    launch_eval_or_lean(st, ep, b->lean_ids.p, b->n_lean, has_live);
+    launch_eval_or_lean(st, ep, b->ids[kRouteLean].p, b->n_ids[kRouteLean], has_live);
     RG_CUDA_CHECK(cudaGetLastError());
-    launch_eval_or_ms(st, ep, b->ms_ids.p, b->n_ms, b->max_ms_streams, has_live, b->uses_planes);
+    launch_eval_or_ms(st, ep, b->ids[kRouteMs].p, b->n_ids[kRouteMs], b->width[kRouteMs], has_live, b->uses_planes);
     RG_CUDA_CHECK(cudaGetLastError());
-    launch_eval_or(st, ep, b->or_ids.p, b->n_or, b->max_or_terms, has_live, b->or_has_not, b->or_has_msm, b->or_has_dmax,
-                   !b->or_nonpos);
+    launch_eval_or(st, ep, b->ids[kRouteOr].p, b->n_ids[kRouteOr], std::max(1u, b->width[kRouteOr]), has_live, b->or_has_not,
+                   b->or_has_msm, b->or_has_dmax, !b->or_nonpos);
     RG_CUDA_CHECK(cudaGetLastError());
-    launch_eval_dpq(st, ep, b->dpq_ids.p, b->n_dpq, b->max_dpq_terms, has_live);
+    launch_eval_dpq(st, ep, b->ids[kRouteDpq].p, b->n_ids[kRouteDpq], b->width[kRouteDpq], has_live);
     RG_CUDA_CHECK(cudaGetLastError());
-    launch_eval_and(st, ep, b->and_ids.p, b->n_and, false, has_other);
+    launch_eval_and(st, ep, b->ids[kRouteAnd].p, b->n_ids[kRouteAnd], false, has_other);
     RG_CUDA_CHECK(cudaGetLastError());
-    launch_eval_and(st, ep, b->ro_ids.p, b->n_ro, true, has_other);
+    launch_eval_and(st, ep, b->ids[kRouteReqOpt].p, b->n_ids[kRouteReqOpt], true, has_other);
     RG_CUDA_CHECK(cudaGetLastError());
     const RangeParams rgp{b->range_refs.p, b->range_stats.p};
-    launch_eval_and_ranges(st, ep, rgp, b->and_rng_ids.p, b->n_and_rng, false, has_other);
+    launch_eval_and_ranges(st, ep, rgp, b->ids[kRouteAndRanges].p, b->n_ids[kRouteAndRanges], false, has_other);
     RG_CUDA_CHECK(cudaGetLastError());
-    launch_eval_and_ranges(st, ep, rgp, b->ro_rng_ids.p, b->n_ro_rng, true, has_other);
+    launch_eval_and_ranges(st, ep, rgp, b->ids[kRouteReqOptRanges].p, b->n_ids[kRouteReqOptRanges], true, has_other);
     RG_CUDA_CHECK(cudaGetLastError());
-    launch_eval_and_nested(st, ep, rgp, b->group_stats.p, b->and_grp_ids.p, b->n_and_grp, false, has_other);
+    launch_eval_and_nested(st, ep, rgp, b->group_stats.p, b->ids[kRouteAndNested].p, b->n_ids[kRouteAndNested], false, has_other);
     RG_CUDA_CHECK(cudaGetLastError());
-    launch_eval_and_nested(st, ep, rgp, b->group_stats.p, b->ro_grp_ids.p, b->n_ro_grp, true, has_other);
+    launch_eval_and_nested(st, ep, rgp, b->group_stats.p, b->ids[kRouteReqOptNested].p, b->n_ids[kRouteReqOptNested], true, has_other);
     RG_CUDA_CHECK(cudaGetLastError());
     RG_CUDA_CHECK(cudaEventRecord(b->ev[3], st));
     ReplayParams rp{};
@@ -2250,81 +2112,73 @@ int rg_batch_stats(rg_engine* e, rg_batch* b, uint64_t out[8]) {
     out[3] = used;
     out[4] = b->kernels_per_run;
     out[5] = b->h2d_bytes;
-    out[6] = b->n_or + b->n_lean + b->n_ms + b->n_dpq;
-    out[7] = b->n_and + b->n_ro;
+    out[6] = b->n_ids[kRouteOr] + b->n_ids[kRouteMs] + b->n_ids[kRouteLean] + b->n_ids[kRouteDpq];
+    out[7] = b->n_ids[kRouteAnd] + b->n_ids[kRouteReqOpt];
     return RG_OK;
     RG_CATCH
 }
 
-int rg_search_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries,
-                    const rg_clause* clauses, uint32_t n_clauses, const rg_search_params* p,
-                    rg_hit* out_hits, uint32_t* out_counts, uint64_t* out_total_hits) {
+// Prepare, run and fetch.  When the candidate arena overflows, the two halves of the batch run one after the other
+// (queries are independent and refer to `clauses` by absolute index, so a half is just a sub-array of `queries`),
+// recursively if need be.
+static int search_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                        uint32_t n_clauses, const rg_search_params* p, const rg_point_range* ranges, uint32_t n_ranges,
+                        const rg_query* groups, uint32_t n_groups, rg_hit* out_hits, uint32_t* out_counts,
+                        uint64_t* out_total_hits) {
     rg_batch* b = nullptr;
-    int rc = rg_batch_prepare(e, queries, n_queries, clauses, n_clauses, p, &b);
+    int rc = batch_prepare(e, queries, n_queries, clauses, n_clauses, p, ranges, n_ranges, &b, groups, n_groups);
     if (rc != RG_OK) return rc;
     rc = rg_batch_run(e, b);
     if (rc == RG_OK) rc = rg_batch_fetch(e, b, out_hits, out_counts, out_total_hits);
     rg_batch_destroy(e, b);
     if (rc == RG_ENOMEM && n_queries > 1 && p && p->k) {
-        // the candidate arena overflowed: the two halves of the batch, one after the other (queries are independent and
-        // refer to `clauses` by absolute index, so a half is just a sub-array of `queries`); recursively if need be
         const uint32_t h = n_queries / 2;
-        rc = rg_search_batch(e, queries, h, clauses, n_clauses, p, out_hits, out_counts, out_total_hits);
+        rc = search_batch(e, queries, h, clauses, n_clauses, p, ranges, n_ranges, groups, n_groups, out_hits, out_counts,
+                          out_total_hits);
         if (rc == RG_OK)
-            rc = rg_search_batch(e, queries + h, n_queries - h, clauses, n_clauses, p, out_hits + (size_t)h * p->k, out_counts + h,
-                                 out_total_hits + h);
+            rc = search_batch(e, queries + h, n_queries - h, clauses, n_clauses, p, ranges, n_ranges, groups, n_groups,
+                              out_hits + (size_t)h * p->k, out_counts + h, out_total_hits + h);
     }
     return rc;
+}
+
+int rg_search_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries,
+                    const rg_clause* clauses, uint32_t n_clauses, const rg_search_params* p,
+                    rg_hit* out_hits, uint32_t* out_counts, uint64_t* out_total_hits) {
+    return search_batch(e, queries, n_queries, clauses, n_clauses, p, nullptr, 0, nullptr, 0, out_hits, out_counts,
+                        out_total_hits);
 }
 
 int rg_search_batch_ranges(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
                            uint32_t n_clauses, const rg_search_params* p, const rg_point_range* ranges,
                            uint32_t n_ranges, rg_hit* out_hits, uint32_t* out_counts, uint64_t* out_total_hits) {
-    rg_batch* b = nullptr;
-    int rc = rg_batch_prepare_ranges(e, queries, n_queries, clauses, n_clauses, p, ranges, n_ranges, &b);
-    if (rc != RG_OK) return rc;
-    rc = rg_batch_run(e, b);
-    if (rc == RG_OK) rc = rg_batch_fetch(e, b, out_hits, out_counts, out_total_hits);
-    rg_batch_destroy(e, b);
-    if (rc == RG_ENOMEM && n_queries > 1 && p && p->k) {  // as rg_search_batch
-        const uint32_t h = n_queries / 2;
-        rc = rg_search_batch_ranges(e, queries, h, clauses, n_clauses, p, ranges, n_ranges, out_hits, out_counts,
-                                    out_total_hits);
-        if (rc == RG_OK)
-            rc = rg_search_batch_ranges(e, queries + h, n_queries - h, clauses, n_clauses, p, ranges, n_ranges,
-                                        out_hits + (size_t)h * p->k, out_counts + h, out_total_hits + h);
-    }
-    return rc;
+    if (!readable(ranges, n_ranges)) return null_argument(nullptr);
+    return search_batch(e, queries, n_queries, clauses, n_clauses, p, ranges, n_ranges, nullptr, 0, out_hits, out_counts,
+                        out_total_hits);
 }
 
 int rg_search_batch_nested(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
                            uint32_t n_clauses, const rg_search_params* p, const rg_point_range* ranges,
                            uint32_t n_ranges, const rg_query* groups, uint32_t n_groups, rg_hit* out_hits,
                            uint32_t* out_counts, uint64_t* out_total_hits) {
-    rg_batch* b = nullptr;
-    int rc = rg_batch_prepare_nested(e, queries, n_queries, clauses, n_clauses, p, ranges, n_ranges, groups, n_groups, &b);
-    if (rc != RG_OK) return rc;
-    rc = rg_batch_run(e, b);
-    if (rc == RG_OK) rc = rg_batch_fetch(e, b, out_hits, out_counts, out_total_hits);
-    rg_batch_destroy(e, b);
-    if (rc == RG_ENOMEM && n_queries > 1 && p && p->k) {  // as rg_search_batch
-        const uint32_t h = n_queries / 2;
-        rc = rg_search_batch_nested(e, queries, h, clauses, n_clauses, p, ranges, n_ranges, groups, n_groups, out_hits,
-                                    out_counts, out_total_hits);
-        if (rc == RG_OK)
-            rc = rg_search_batch_nested(e, queries + h, n_queries - h, clauses, n_clauses, p, ranges, n_ranges, groups,
-                                        n_groups, out_hits + (size_t)h * p->k, out_counts + h, out_total_hits + h);
-    }
-    return rc;
+    if (!readable(ranges, n_ranges) || !readable(groups, n_groups)) return null_argument(nullptr);
+    return search_batch(e, queries, n_queries, clauses, n_clauses, p, ranges, n_ranges, groups, n_groups, out_hits,
+                        out_counts, out_total_hits);
 }
+
+// n counters of the batch's last run (zeros before it has run)
+static void copy_counters(rg_engine* e, const rg_batch* b, const Span<unsigned long long>& src, uint64_t* out, size_t n) {
+    memset(out, 0, n * sizeof(uint64_t));
+    if (b->ran) {
+        RG_CUDA_CHECK(cudaStreamSynchronize(e->stream));
+        RG_CUDA_CHECK(cudaMemcpy(out, src.p, n * sizeof(uint64_t), cudaMemcpyDeviceToHost));
+    }
+}
+
 int rg_batch_range_stats(rg_engine* e, rg_batch* b, uint64_t out[3]) {
     RG_TRY
     if (!e || !b || !out) throw ArgError("null argument");
-    memset(out, 0, 3 * sizeof(uint64_t));
-    if (b->ran) {
-        RG_CUDA_CHECK(cudaStreamSynchronize(e->stream));
-        RG_CUDA_CHECK(cudaMemcpy(out, b->range_stats.p, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-    }
+    copy_counters(e, b, b->range_stats, out, 3);
     return RG_OK;
     RG_CATCH
 }
@@ -2332,11 +2186,7 @@ int rg_batch_range_stats(rg_engine* e, rg_batch* b, uint64_t out[3]) {
 int rg_batch_group_stats(rg_engine* e, rg_batch* b, uint64_t out[3]) {
     RG_TRY
     if (!e || !b || !out) throw ArgError("null argument");
-    memset(out, 0, 3 * sizeof(uint64_t));
-    if (b->ran) {
-        RG_CUDA_CHECK(cudaStreamSynchronize(e->stream));
-        RG_CUDA_CHECK(cudaMemcpy(out, b->group_stats.p, 3 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-    }
+    copy_counters(e, b, b->group_stats, out, 3);
     return RG_OK;
     RG_CATCH
 }
@@ -2344,12 +2194,8 @@ int rg_batch_group_stats(rg_engine* e, rg_batch* b, uint64_t out[3]) {
 int rg_batch_debug(rg_engine* e, rg_batch* b, uint64_t out[16]) {
     RG_TRY
     if (!e || !b || !out) throw ArgError("null argument");
-    memset(out, 0, 16 * sizeof(uint64_t));
-    if (b->ran) {
-        RG_CUDA_CHECK(cudaStreamSynchronize(e->stream));
-        RG_CUDA_CHECK(cudaMemcpy(out, b->dbg.p, 16 * sizeof(uint64_t), cudaMemcpyDeviceToHost));
-    }
-    out[14] = b->n_lean;
+    copy_counters(e, b, b->dbg, out, 16);
+    out[14] = b->n_ids[kRouteLean];
     return RG_OK;
     RG_CATCH
 }
