@@ -339,6 +339,19 @@ int rg_batch_rescore(rg_engine* e, rg_batch* b, const rg_query* queries, uint32_
 int rg_rescore_hits(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
                     uint32_t n_clauses, const rg_rescore_params* p, uint32_t k, rg_hit* hits,
                     const uint32_t* counts, const uint64_t* total_hits);
+/* rg_batch_rescore / rg_rescore_hits for rescoring queries with point ranges (RG_CLAUSE_RANGE) and nested groups
+ * (RG_CLAUSE_GROUP), the `ranges` / `groups` arrays as rg_batch_prepare_nested takes them (either may be NULL with a
+ * count of 0).  Accepted: every shape rg_batch_prepare_nested accepts, except the ones rescoring refuses above (a
+ * group of 10 or more members that is the whole query scores through a DisiPriorityQueue too).  RG_EUNSUPPORTED and
+ * RG_EINVAL as rg_batch_prepare_nested gives them for the shape, and as rg_batch_rescore / rg_rescore_hits give them
+ * for the rows; on any error the rows are untouched.  rg_engine_last_kernel_ms(e, "rescore") times these launches too. */
+int rg_batch_rescore_nested(rg_engine* e, rg_batch* b, const rg_query* queries, uint32_t n_queries,
+                            const rg_clause* clauses, uint32_t n_clauses, const rg_point_range* ranges,
+                            uint32_t n_ranges, const rg_query* groups, uint32_t n_groups, const rg_rescore_params* p);
+int rg_rescore_hits_nested(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                           uint32_t n_clauses, const rg_point_range* ranges, uint32_t n_ranges, const rg_query* groups,
+                           uint32_t n_groups, const rg_rescore_params* p, uint32_t k, rg_hit* hits,
+                           const uint32_t* counts, const uint64_t* total_hits);
 
 /* Sharded mode (one segment per GPU).  After rg_batch_run with RG_MODE_SEARCH_PARALLEL the
  * per-query leaf record {uint32 n; uint32 pad; uint64 total_hits; rg_hit heap[k]} (heap-array

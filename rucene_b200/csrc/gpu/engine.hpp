@@ -261,8 +261,10 @@ void launch_eval_and_nested(cudaStream_t st, const EvalParams& p, const RangePar
 
 // rescore.cu: QueryRescorer over TopDocs rows in HBM.  The rescoring query's scorer per (query, leaf), as
 // BooleanWeight::create_scorer builds it; its clauses are ItemClauses (weight = the clause's scoring weight, flags
-// bit0 MUST_NOT, bit1 optional side of a ReqOptScorer), required ones first (conjunctions in cost order), then the
-// optional ones, then the MUST_NOT ones, each group in clause order.
+// kClauseNot for MUST_NOT, kClauseOpt for the optional side of a ReqOptScorer), required ones first (conjunctions in
+// cost order), then the optional ones, then the MUST_NOT ones, each group in clause order.  k_rescore<true> also
+// takes group members (kClauseReqGroup / kClauseOptGroup / kClauseGroupLast, counted one by one in n_req / n_opt) and
+// point ranges (kClauseRange, with kClauseNot when excluded; term_id indexes RescoreParams::ranges).
 enum : uint8_t {
     kRsNone = 0,  // create_scorer returned None: nothing matches in this leaf
     kRsTerm = 1,  // TermScorer (a bare TermQuery, or what BooleanQuery::build / DisjunctionMaxQuery collapse to)
@@ -289,9 +291,11 @@ struct RescoreParams {
     uint32_t n_queries, k, window, mode;
     float query_weight, rescore_weight;
     uint32_t ncap;              // power of two >= min(k, window), >= 32: shared-memory slots per query
+    const RangeRef* ranges;     // k_rescore<true>: RangeRef per (leaf, range), leaf-major
 };
-size_t rescore_smem_bytes(uint32_t ncap);
-void launch_rescore(cudaStream_t st, const RescoreParams& p);
+size_t rescore_smem_bytes(uint32_t ncap, bool nested);
+// nested: k_rescore<true> (the plan has group or range clauses)
+void launch_rescore(cudaStream_t st, const RescoreParams& p, bool nested);
 
 struct ReplayParams {
     const rg_hit* cand_arena;

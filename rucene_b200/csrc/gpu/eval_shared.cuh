@@ -347,6 +347,19 @@ __device__ __forceinline__ bool is_live(const SegDev& seg, int doc) {
     return (seg.live[doc >> 6] >> (doc & 63)) & 1ull;
 }
 
+// PointRangeIntersectVisitor::visit_by_packed_value over every value of doc d: lower <= key <= upper for any of
+// them (keys ascending within a doc)
+__device__ __forceinline__ bool range_hit(const RangeRef& r, int d) {
+    const uint32_t o0 = __ldg(r.offsets + d), o1 = __ldg(r.offsets + d + 1);
+    for (uint32_t j = o0; j < o1; j++) {
+        const uint64_t key = r.wide ? __ldg(static_cast<const unsigned long long*>(r.keys) + j)
+                                    : (uint64_t)__ldg(static_cast<const uint32_t*>(r.keys) + j);
+        if (key > r.upper) return false;
+        if (key >= r.lower) return true;
+    }
+    return false;
+}
+
 // ------------------------------------------------------------------------------------------
 // k_eval_or  — one WARP per work item, no block-level synchronisation at all.
 // ------------------------------------------------------------------------------------------

@@ -618,19 +618,6 @@ struct AndSharedN : AndSharedR {
     int32_t gx;                         // this step merges docids from gx on
 };
 
-// PointRangeIntersectVisitor::visit_by_packed_value over every value of doc d: lower <= key <= upper for any of
-// them (keys ascending within a doc)
-__device__ __forceinline__ bool range_hit(const RangeRef& r, int d) {
-    const uint32_t o0 = __ldg(r.offsets + d), o1 = __ldg(r.offsets + d + 1);
-    for (uint32_t j = o0; j < o1; j++) {
-        const uint64_t key = r.wide ? __ldg(static_cast<const unsigned long long*>(r.keys) + j)
-                                    : (uint64_t)__ldg(static_cast<const uint32_t*>(r.keys) + j);
-        if (key > r.upper) return false;
-        if (key >= r.lower) return true;
-    }
-    return false;
-}
-
 // OTHER: some leaf carries EF / BITSET doc blocks (their decoder is compiled out otherwise).
 // RANGES: the item has point-range clauses (kClauseRange); a range that leads walks the item's docids one 128-doc
 // block per warp.  Without it the body is the plain conjunction / ReqOpt kernel, unchanged.

@@ -9,6 +9,12 @@
 // with the first-pass score (combine_score :349-367), the window is sorted by (score desc, docid asc)
 // (ScoreDocHit's Ord, sort_field/collapse_top_docs.rs:180-201) and written back; every hit after the window is
 // scaled by query_weight (combine_docs :375-417).
+//
+// k_rescore<true> is the same walk for rescoring queries with pure-SHOULD groups (kClauseReqGroup / kClauseOptGroup,
+// members contiguous and in member order, kClauseGroupLast on the last) and point ranges (kClauseRange: term_id
+// indexes RescoreParams::ranges per (leaf, range)).  A group's members add into a per-target DisjunctionSumScorer sum
+// (from 0.0f); after its last member the sum folds into the group's side as one value.  A required range counts as one
+// required clause that adds +0.0f; a MUST_NOT range excludes.  k_rescore<false> compiles none of that code.
 #include "eval_shared.cuh"
 
 namespace rg {
@@ -19,6 +25,7 @@ constexpr uint32_t kRsReqAny = 1u;   // some scoring clause of the required side
 constexpr uint32_t kRsOptAny = 2u;   // some optional (ReqOptScorer) clause has it
 constexpr uint32_t kRsExcl = 4u;     // some MUST_NOT clause has it (ReqNotScorer)
 constexpr uint32_t kRsCountSh = 8u;  // bits [8, 16): required clauses that have it (conjunctions)
+constexpr uint32_t kRsGroupAny = 1u << 16;  // some member of the group being walked has it (k_rescore<true>)
 constexpr uint32_t kRsMatched = 0x80000000u;  // the leaf's scorer matched the target
 constexpr uint32_t kRsOptThreshold = 100;     // ReqOptScorer: scores_num above which low scores skip the optional side
 
@@ -59,7 +66,9 @@ __device__ __forceinline__ float combine(uint32_t mode, float a, float b) {
 }
 
 // One clause over the targets keys[b, e) (ascending global docids in the high words) of one leaf: the
-// scorer's advance(target) for each, as a forward walk.  Updates acc / acc2 / st of the targets it finds.
+// scorer's advance(target) for each, as a forward walk.  Updates acc / acc2 / st of the targets it finds.  NESTED: a
+// group member adds into the target's group sum (the ncap floats after bfreqs) and flags it kRsGroupAny.
+template <bool NESTED>
 __device__ void probe_clause(const RescoreParams& p, const SegDev& seg, const ItemClause c, uint32_t ci,
                              uint32_t kind, const unsigned long long* keys, uint32_t b, uint32_t e, float* acc,
                              float* acc2, uint32_t* st, int32_t* bdocs, int32_t* bfreqs, int lane) {
@@ -115,7 +124,11 @@ __device__ void probe_clause(const RescoreParams& p, const SegDev& seg, const It
                 if (l < n_in && bdocs[l] == dj) {
                     const float nrm = seg.norms ? __ldg(cache + __ldg(seg.norms + dj)) : p.k1;
                     const float s = bm25_score(w1, (float)bfreqs[l], nrm);
-                    if (role == kClauseNot) {
+                    if (NESTED && (c.flags & (kClauseReqGroup | kClauseOptGroup))) {
+                        float* gsum = reinterpret_cast<float*>(bfreqs + kBlock);
+                        gsum[j] = __fadd_rn(gsum[j], s);  // DisjunctionSumScorer from 0.0f, member order
+                        st[j] |= kRsGroupAny;
+                    } else if (role == kClauseNot) {
                         st[j] |= kRsExcl;
                     } else if (role == kClauseOpt) {
                         acc2[j] = __fadd_rn(acc2[j], s);  // DisjunctionSumScorer from 0.0f, clause order
@@ -144,9 +157,34 @@ __device__ void probe_clause(const RescoreParams& p, const SegDev& seg, const It
     __syncwarp();
 }
 
+// PointRangeWeight's scorer over the targets keys[b, e) of one leaf (k_rescore<true>): a target's RangeBlock rules
+// out a block wholly outside the range, takes a doc with a value in a block wholly inside it, and sends the rest to
+// the doc's keys.  A required range counts as one required clause and adds +0.0f at position ci (a -0.0f sum becomes
+// +0.0f, as in the reference); a MUST_NOT range excludes.
+__device__ void probe_range(const RangeRef& rr, const SegDev& seg, uint32_t ci, bool excl,
+                            const unsigned long long* keys, uint32_t b, uint32_t e, float* acc, uint32_t* st, int lane) {
+    for (uint32_t j = b + lane; j < e; j += 32) {
+        const int d = (int)(keys[j] >> 32) - seg.doc_base;
+        const RangeBlock bk = rr.blocks[d / kBlock];
+        if (bk.values == 0 || bk.max < rr.lower || bk.min > rr.upper) continue;
+        const bool hit = bk.min >= rr.lower && bk.max <= rr.upper ? __ldg(rr.offsets + d + 1) > __ldg(rr.offsets + d)
+                                                                  : range_hit(rr, d);
+        if (!hit) continue;
+        if (excl) {
+            st[j] |= kRsExcl;
+        } else {
+            acc[j] = ci == 0 ? 0.0f : __fadd_rn(acc[j], 0.0f);
+            st[j] += 1u << kRsCountSh;
+        }
+    }
+    __syncwarp();
+}
+
 }  // namespace
 
-// named outside the anonymous namespace so that its symbol (profiler traces) is stable across builds
+// named outside the anonymous namespace so that its symbols (profiler traces) are stable across builds.  NESTED: the
+// plan has group or range clauses; only nested or range rescoring launches k_rescore<true>
+template <bool NESTED>
 __global__ void __launch_bounds__(32) k_rescore(RescoreParams p) {
     extern __shared__ __align__(16) unsigned char smem_raw[];
     const uint32_t q = blockIdx.x;
@@ -159,6 +197,7 @@ __global__ void __launch_bounds__(32) k_rescore(RescoreParams p) {
     uint32_t* st = reinterpret_cast<uint32_t*>(acc2 + ncap);
     int32_t* bdocs = reinterpret_cast<int32_t*>(st + ncap);
     int32_t* bfreqs = bdocs + kBlock;
+    float* gsum = reinterpret_cast<float*>(bfreqs + kBlock);  // NESTED: the group sum of each target
 
     const uint32_t cnt = min(p.counts[q], p.k);
     if (p.totals[q] == 0 || cnt == 0) return;  // nothing changes, not even the tail (rescorer.rs:130-140)
@@ -176,6 +215,7 @@ __global__ void __launch_bounds__(32) k_rescore(RescoreParams p) {
         acc[i] = 0.0f;
         acc2[i] = 0.0f;
         st[i] = 0u;
+        if (NESTED) gsum[i] = 0.0f;
     }
     __syncwarp();
 
@@ -202,9 +242,53 @@ __global__ void __launch_bounds__(32) k_rescore(RescoreParams p) {
                 for (uint32_t i = b + lane; i < e; i += 32) acc2[i] = -INFINITY;
             __syncwarp();
             const uint32_t n_cl = (uint32_t)L.n_req + L.n_opt + L.n_not;
-            for (uint32_t ci = 0; ci < n_cl; ci++)
-                probe_clause(p, seg, p.clauses[L.clause_begin + ci], ci, L.kind, keys, b, e, acc, acc2, st, bdocs,
-                             bfreqs, lane);
+            // NESTED: n_req counts group members one by one; a conjunction needs each required term, range and group
+            // once.  g0: the first clause of the group being walked (the group is the first summand when it is 0)
+            uint32_t need = L.n_req, g0 = 0;
+            if (!NESTED) {
+                for (uint32_t ci = 0; ci < n_cl; ci++)
+                    probe_clause<false>(p, seg, p.clauses[L.clause_begin + ci], ci, L.kind, keys, b, e, acc, acc2, st,
+                                        bdocs, bfreqs, lane);
+            } else {
+                need = 0;
+            }
+            for (uint32_t ci = 0; NESTED && ci < n_cl; ci++) {
+                const ItemClause c = p.clauses[L.clause_begin + ci];
+                if (NESTED && (c.flags & kClauseRange)) {
+                    probe_range(p.ranges[c.term_id], seg, ci, (c.flags & kClauseNot) != 0, keys, b, e, acc, st, lane);
+                    need += (c.flags & kClauseNot) ? 0u : 1u;
+                    g0 = ci + 1;
+                    continue;
+                }
+                probe_clause<true>(p, seg, c, ci, L.kind, keys, b, e, acc, acc2, st, bdocs, bfreqs, lane);
+                const uint32_t side = c.flags & (kClauseReqGroup | kClauseOptGroup);
+                if (!side) {
+                    need += (c.flags & (kClauseNot | kClauseOpt)) ? 0u : 1u;
+                    g0 = ci + 1;
+                    continue;
+                }
+                if (!(c.flags & kClauseGroupLast)) continue;
+                // the group's DisjunctionSumScorer landed on the targets some member has: a required group is one
+                // summand of the conjunction (cost order), an optional one one summand of the optional side (clause
+                // order); then its sums start again from 0.0f
+                for (uint32_t i = b + lane; i < e; i += 32) {
+                    const uint32_t s = st[i];
+                    if (s & kRsGroupAny) {
+                        const float v = gsum[i];
+                        if (side == kClauseReqGroup) {
+                            acc[i] = g0 == 0 ? v : __fadd_rn(acc[i], v);
+                            st[i] = (s & ~kRsGroupAny) + (1u << kRsCountSh);
+                        } else {
+                            acc2[i] = __fadd_rn(acc2[i], v);
+                            st[i] = (s & ~kRsGroupAny) | kRsOptAny;
+                        }
+                        gsum[i] = 0.0f;
+                    }
+                }
+                __syncwarp();
+                need += side == kClauseReqGroup ? 1u : 0u;
+                g0 = ci + 1;
+            }
             // the per-target scorer result: matched flag in st bit 31, score in acc
             for (uint32_t i = b + lane; i < e; i += 32) {
                 const uint32_t s = st[i];
@@ -214,7 +298,7 @@ __global__ void __launch_bounds__(32) k_rescore(RescoreParams p) {
                     m = true;
                     v = 0.0f;
                 } else if (L.kind == kRsConj) {
-                    m = (s >> kRsCountSh) == L.n_req;
+                    m = (s >> kRsCountSh) == need;
                 } else {
                     m = (s & kRsReqAny) != 0;
                     if (L.kind == kRsMax) v = __fadd_rn(acc2[i], __fmul_rn(__fsub_rn(v, acc2[i]), L.tie));
@@ -263,14 +347,17 @@ __global__ void __launch_bounds__(32) k_rescore(RescoreParams p) {
     }
 }
 
-size_t rescore_smem_bytes(uint32_t ncap) {
-    return (size_t)ncap * (8 + 8 + 4 + 4 + 4) + 2 * kBlock * sizeof(int32_t);
+
+size_t rescore_smem_bytes(uint32_t ncap, bool nested) {
+    return (size_t)ncap * (8 + 8 + 4 + 4 + 4 + (nested ? 4 : 0)) + 2 * kBlock * sizeof(int32_t);
 }
 
-void launch_rescore(cudaStream_t st, const RescoreParams& p) {
+void launch_rescore(cudaStream_t st, const RescoreParams& p, bool nested) {
     if (p.n_queries == 0) return;
-    const size_t smem = rescore_smem_bytes(p.ncap);  // at most 29.7 KB (ncap 1024): no opt-in above 48 KB needed
-    k_rescore<<<p.n_queries, 32, smem, st>>>(p);
+    // at most 33.8 KB (ncap 1024, nested): no opt-in above 48 KB needed
+    const size_t smem = rescore_smem_bytes(p.ncap, nested);
+    if (nested) k_rescore<true><<<p.n_queries, 32, smem, st>>>(p);
+    else k_rescore<false><<<p.n_queries, 32, smem, st>>>(p);
 }
 
 }  // namespace rg

@@ -591,6 +591,74 @@ bool resolve_ranges(const QShape& shape, const Segment& seg, const rg_clause* cl
     return true;
 }
 
+// BooleanWeight::create_scorer of a conjunction / ReqOpt shape (kTypeAnd / kTypeReqOpt) in one leaf, for the first pass
+// (plan_batch) and rescoring (plan_rescore) alike.  A term's cost() is its doc_freq.  A group is a
+// DisjunctionSumScorer over its members present here (even over one: the `1 =>` arm is commented out,
+// boolean_query.rs:196-279), None when it has none; its cost() is the sum of those members' doc_freq
+// (disjunction_scorer.rs:39).  A required clause that is None leaves the leaf without a scorer (:201-206), an optional
+// one is left out (:217-234).  MUST_NOT groups arrive flattened (classify_groups).
+struct ConjLeaf {
+    // a required / optional clause in this leaf: its clauses here are members[begin, begin + n)
+    struct Req {
+        uint64_t cost;
+        uint32_t begin, n;
+        bool group, filter;
+    };
+    std::vector<Req> req, opt;    // req: ConjunctionScorer's cost order (stable); opt: clause order
+    std::vector<uint32_t> members, nots, rnots;  // nots: MUST_NOT terms present here; rnots: MUST_NOT ranges
+    std::vector<std::pair<uint64_t, uint32_t>> rreq;  // required ranges with their point counts, cheapest first
+    bool range_lead = false;      // a range leads (cheaper than every term and group)
+    uint32_t leaf_type = 0;       // kTypeReqOpt only when some optional clause has a scorer here
+    uint64_t cost = 0;            // the lead's
+
+    // false: the leaf has no scorer
+    bool resolve(const QShape& shape, const Segment& seg, const rg_clause* clauses, const rg_point_range* ranges) {
+        auto df_of = [&](uint32_t ci) -> uint64_t {
+            const uint32_t t = clauses[ci].term_id;
+            return t < seg.host_terms.size() && seg.host_terms[t].doc_freq > 0 ? (uint64_t)seg.host_terms[t].doc_freq : 0;
+        };
+        auto entry = [&](const QShape::Entry& en) {
+            Req r{0, (uint32_t)members.size(), 0, en.group, en.filter};
+            for (uint32_t j = 0; j < en.n; j++)
+                if (const uint64_t df = df_of(en.begin + j)) {
+                    members.push_back(en.begin + j);
+                    r.cost += df;
+                }
+            r.n = (uint32_t)members.size() - r.begin;
+            return r;
+        };
+        req.clear();
+        opt.clear();
+        members.clear();
+        nots.clear();
+        rreq.clear();
+        rnots.clear();
+        bool dead = shape.req_seq.empty() && shape.req_rng.empty();
+        for (const QShape::Entry& en : shape.req_seq) {
+            req.push_back(entry(en));
+            dead = dead || req.back().n == 0;
+        }
+        if (dead) return false;
+        for (const QShape::Entry& en : shape.opt_seq) {
+            const Req r = entry(en);
+            if (r.n) opt.push_back(r);
+        }
+        for (uint32_t ci : shape.not_idx)
+            if (df_of(ci)) nots.push_back(ci);
+        // point ranges: the required ones with their point counts (cheapest first) and the MUST_NOT ones
+        if ((!shape.req_rng.empty() || !shape.not_rng.empty()) && !resolve_ranges(shape, seg, clauses, ranges, rreq, rnots))
+            return false;
+        // ConjunctionScorer::new: stable sort by cost() (:30); the score is lead1 + lead2 + the others in that
+        // order, each group one f32 value
+        std::stable_sort(req.begin(), req.end(), [](const Req& a, const Req& b) { return a.cost < b.cost; });
+        range_lead = !rreq.empty() && (req.empty() || rreq[0].first < req[0].cost);
+        // no SHOULD scorer in this leaf -> the MUST side alone, no ReqOptScorer (:259-266)
+        leaf_type = shape.type == kTypeReqOpt && opt.empty() ? (uint32_t)kTypeAnd : (uint32_t)shape.type;
+        cost = range_lead ? rreq[0].first : req[0].cost;
+        return true;
+    }
+};
+
 // Score columns: which (leaf, term, weight, norm cache, k1) clauses of the batch's disjunctions are read
 // from a materialised f32 column (k_build_columns) instead of their block stream.  Only terms with a
 // presence bitmap (df >= max_doc/64, chosen at upload) qualify.  Columns are persistent: a key that is
@@ -1141,28 +1209,69 @@ void choose_local_lists(rg_engine* e, const std::vector<QShape>& shapes, const r
     }
 }
 
+// The shape of every query of a batch: classify_groups where the entry point passes groups, classify_ranges where it
+// passes ranges, else classify (rescore: with the refusals of rescoring queries).  With groups, `ext` is the planner's copy of the
+// clause array plus what the collapses append; returns the clause array the shapes index.
+const rg_clause* classify_batch(const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                                uint32_t n_clauses, const rg_point_range* ranges, uint32_t n_ranges,
+                                const rg_query* groups, uint32_t n_groups, uint32_t n_caches, bool rescore,
+                                std::vector<rg_clause>& ext, std::vector<QShape>& shapes) {
+    shapes.assign(n_queries, QShape{});
+    if (groups) ext.assign(clauses, clauses + n_clauses);
+    for (uint32_t qi = 0; qi < n_queries; qi++) {
+        if (ranges && (uint64_t)queries[qi].clause_begin + queries[qi].n_clauses > n_clauses)
+            throw ArgError("query clause range out of bounds");
+        if (groups && classify_groups(queries[qi], ext, n_clauses, ranges, n_ranges, groups, n_groups, n_caches, shapes[qi])) {
+        } else if (ranges && classify_ranges(queries[qi], groups ? ext.data() : clauses, ranges, n_ranges, shapes[qi])) {
+        } else {
+            shapes[qi] = classify(queries[qi], groups ? ext.data() : clauses, n_clauses, rescore);
+        }
+        if (groups) clauses = ext.data();  // (ext may have moved)
+        const QShape& sh = shapes[qi];
+        // ReqNotScorer moves past an excluded hit with next(), and a SHOULD disjunction with min_should_match > 1
+        // then skips to the next doc that reaches min_should_match: whether a later hit matches depends on the walk
+        if (rescore && sh.msm > 1 && !sh.not_idx.empty())
+            throw Unsupported("rescoring with a min_should_match > 1 disjunction beside MUST_NOT clauses");
+        // a query that is a group of 10 or more members scores through a DisiPriorityQueue (classify refuses the
+        // flat shapes of that width)
+        if (rescore && sh.type == kTypeOr && sh.msm == 0 && sh.clause_idx.size() > (size_t)kMaxTerms)
+            throw Unsupported("rescoring with a disjunction of 10 or more clauses and min_should_match <= 1 (DisiPriorityQueue order)");
+        check_caches(sh, clauses, n_caches);
+    }
+    return clauses;
+}
+
+// RangeRef per (leaf, range), leaf-major: the range clauses of leaf si point at entry si * n_ranges + range
+void fill_range_refs(const rg_engine* e, const rg_point_range* ranges, uint32_t n_ranges, std::vector<RangeRef>& refs) {
+    const uint32_t n_segs = (uint32_t)e->segs.size();
+    refs.assign((size_t)n_segs * n_ranges, RangeRef{});
+    for (uint32_t si = 0; si < n_segs; si++)
+        for (uint32_t ri = 0; ri < n_ranges; ri++) {
+            const rg_point_range& r = ranges[ri];
+            const PointField* pfp = point_field(e->segs[si], r);  // a bytes_per_dim mismatch is RG_EINVAL here
+            if (!pfp) continue;
+            const PointField& pf = *pfp;
+            refs[(size_t)si * n_ranges + ri] = RangeRef{pf.offsets.p, pf.keys.p, pf.blocks.p, be_key(r.lower, r.bytes_per_dim),
+                                                        be_key(r.upper, r.bytes_per_dim), pf.bytes_per_dim == 8 ? 1u : 0u, 0u};
+        }
+}
+
+bool has_ranges(const std::vector<QShape>& shapes) {
+    for (const QShape& sh : shapes)
+        if (!sh.req_rng.empty() || !sh.not_rng.empty()) return true;
+    return false;
+}
+
 void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
                 uint32_t n_clauses, uint32_t mode, float k1, HostPlan& hp, PlanTimer& tm, PlanScratch& scratch,
                 const rg_point_range* ranges, uint32_t n_ranges, const rg_query* groups = nullptr,
                 uint32_t n_groups = 0) {
     const uint32_t n_caches = (uint32_t)(e->h_caches.size() / 256);
     const uint32_t n_segs = (uint32_t)e->segs.size();
-    std::vector<QShape> shapes(n_queries);
-    bool any_ranges = false;
-    // groups: the clause array grows by what the collapses make (classify_groups)
-    std::vector<rg_clause> ext;
-    if (groups) ext.assign(clauses, clauses + n_clauses);
-    for (uint32_t qi = 0; qi < n_queries; qi++) {
-        if (ranges && (uint64_t)queries[qi].clause_begin + queries[qi].n_clauses > n_clauses)
-            throw ArgError("query clause range out of bounds");
-        if (groups && classify_groups(queries[qi], ext, n_clauses, ranges, n_ranges, groups, n_groups, n_caches, shapes[qi])) {
-            any_ranges = any_ranges || !shapes[qi].req_rng.empty() || !shapes[qi].not_rng.empty();
-        } else if (ranges && classify_ranges(queries[qi], groups ? ext.data() : clauses, ranges, n_ranges, shapes[qi]))
-            any_ranges = true;
-        else shapes[qi] = classify(queries[qi], groups ? ext.data() : clauses, n_clauses);
-        if (groups) clauses = ext.data();  // (ext may have moved)
-        check_caches(shapes[qi], clauses, n_caches);
-    }
+    std::vector<QShape> shapes;
+    std::vector<rg_clause> ext;  // groups: the clause array grows by what the collapses make (classify_groups)
+    clauses = classify_batch(queries, n_queries, clauses, n_clauses, ranges, n_ranges, groups, n_groups, n_caches, false,
+                             ext, shapes);
     // Docid ranges (= work items) per (query, leaf).  A caller's rg_config.range_postings is taken as is: ~that many
     // postings per range.  By default conjunction items (one CTA each) get 32 K postings; disjunctions (one warp each)
     // are cut on a GRID THE WHOLE BATCH SHARES: per leaf a power of two R_leaf <= 256 of equal docid ranges, sized so that
@@ -1196,20 +1305,7 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
             or_grid[si] = std::min<uint32_t>(g, (uint32_t)max_ranges);
         }
     }
-    // every (leaf, range) pair: the range clauses of leaf si point at entry si * n_ranges + range
-    if (any_ranges) {
-        hp.range_refs.assign((size_t)n_segs * n_ranges, RangeRef{});
-        for (uint32_t si = 0; si < n_segs; si++)
-            for (uint32_t ri = 0; ri < n_ranges; ri++) {
-                const rg_point_range& r = ranges[ri];
-                const PointField* pfp = point_field(e->segs[si], r);  // a bytes_per_dim mismatch is RG_EINVAL here
-                if (!pfp) continue;
-                const PointField& pf = *pfp;
-                hp.range_refs[(size_t)si * n_ranges + ri] =
-                    RangeRef{pf.offsets.p, pf.keys.p, pf.blocks.p, be_key(r.lower, r.bytes_per_dim),
-                             be_key(r.upper, r.bytes_per_dim), pf.bytes_per_dim == 8 ? 1u : 0u, 0u};
-            }
-    }
+    if (has_ranges(shapes)) fill_range_refs(e, ranges, n_ranges, hp.range_refs);
     tm.mark("classify");
     const std::map<ColKey, uint32_t> columns = choose_columns(e, shapes, clauses, k1, hp, tm);
     tm.mark("columns");
@@ -1226,16 +1322,10 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
     std::mutex refs_mutex;
     const uint32_t n_threads = n_queries >= 512 ? std::min<uint32_t>(16u, std::max(1u, std::thread::hardware_concurrency())) : 1u;
     auto plan_range = [&](uint32_t q_begin, uint32_t q_end, HostPlan& lp) {
-    // a required / optional clause of a conjunction in one leaf: its clauses there are members[begin, begin + n)
-    struct Req {
-        uint64_t cost;
-        uint32_t begin, n;
-        bool group, filter;
-    };
+    using Req = ConjLeaf::Req;
     // scratch of every (query, leaf) this thread plans
-    std::vector<Req> req, opt;
-    std::vector<uint32_t> members, present, nots, opts, rnots;
-    std::vector<std::pair<uint64_t, uint32_t>> rreq;
+    ConjLeaf cl;
+    std::vector<uint32_t> present, nots, opts;
     for (uint32_t qi = q_begin; qi < q_end; qi++) {
         const QShape& shape = shapes[qi];
         bool group_open = false;
@@ -1280,56 +1370,15 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
             };
             const uint32_t clause_begin = (uint32_t)lp.clauses.size();
             if (shape.type != kTypeOr) {
-                // BooleanWeight::create_scorer of a conjunction / ReqOpt in this leaf.  A term's cost() is its doc_freq.
-                // A group is a DisjunctionSumScorer over its members present here (even over one: the `1 =>` arm is
-                // commented out, boolean_query.rs:196-279), None when it has none; its cost() is the sum of those
-                // members' doc_freq (disjunction_scorer.rs:39).  A required clause that is None leaves the leaf
-                // without a scorer (:201-206), an optional one is left out (:217-234).
-                auto df_of = [&](uint32_t ci) -> uint64_t {
-                    const uint32_t t = clauses[ci].term_id;
-                    return t < seg.host_terms.size() && seg.host_terms[t].doc_freq > 0 ? (uint64_t)seg.host_terms[t].doc_freq : 0;
-                };
-                auto resolve = [&](const QShape::Entry& en) {
-                    Req r{0, (uint32_t)members.size(), 0, en.group, en.filter};
-                    for (uint32_t j = 0; j < en.n; j++)
-                        if (const uint64_t df = df_of(en.begin + j)) {
-                            members.push_back(en.begin + j);
-                            r.cost += df;
-                        }
-                    r.n = (uint32_t)members.size() - r.begin;
-                    return r;
-                };
-                req.clear();
-                opt.clear();
-                members.clear();
-                nots.clear();
-                rreq.clear();
-                rnots.clear();
-                bool dead = shape.req_seq.empty() && shape.req_rng.empty();
-                for (const QShape::Entry& en : shape.req_seq) {
-                    req.push_back(resolve(en));
-                    dead = dead || req.back().n == 0;
-                }
-                if (dead) continue;
-                for (const QShape::Entry& en : shape.opt_seq) {
-                    const Req r = resolve(en);
-                    if (r.n) opt.push_back(r);
-                }
-                for (uint32_t ci : shape.not_idx)
-                    if (df_of(ci)) nots.push_back(ci);
-                // point ranges: the required ones with their point counts (cheapest first) and the MUST_NOT ones
-                if ((!shape.req_rng.empty() || !shape.not_rng.empty()) &&
-                    !resolve_ranges(shape, seg, clauses, ranges, rreq, rnots))
-                    continue;
-                // ConjunctionScorer::new: stable sort by cost() (:30); the score is lead1 + lead2 + the others in that
-                // order, each group one f32 value
-                std::stable_sort(req.begin(), req.end(), [](const Req& a, const Req& b) { return a.cost < b.cost; });
-                // the cheapest required clause leads (a range, whose cost is its point count in the leaf, only when it
-                // is cheaper than every term and group)
-                const bool range_lead = !rreq.empty() && (req.empty() || rreq[0].first < req[0].cost);
-                // no SHOULD scorer in this leaf -> the MUST side alone, no ReqOptScorer (:259-266)
-                const uint32_t leaf_type = shape.type == kTypeReqOpt && opt.empty() ? (uint32_t)kTypeAnd : (uint32_t)shape.type;
-                const uint64_t cost = range_lead ? rreq[0].first : req[0].cost;
+                // BooleanWeight::create_scorer of a conjunction / ReqOpt in this leaf
+                if (!cl.resolve(shape, seg, clauses, ranges)) continue;
+                const std::vector<Req>& req = cl.req;
+                const std::vector<Req>& opt = cl.opt;
+                const std::vector<uint32_t>& members = cl.members;
+                const auto& rreq = cl.rreq;
+                const bool range_lead = cl.range_lead;
+                const uint32_t leaf_type = cl.leaf_type;
+                const uint64_t cost = cl.cost;
                 // bytes: the lead's postings (a range lead: its block table and keys, and every clause's list); each
                 // probed term at most one block per lead doc; a group counts as its members
                 auto enc = [&](uint32_t ci) -> uint64_t { return seg.host_terms[clauses[ci].term_id].enc_bytes; };
@@ -1347,7 +1396,7 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
                     }
                 for (const Req& r : opt)
                     for (uint32_t j = 0; j < r.n; j++) bytes += probed(members[r.begin + j]);
-                for (uint32_t ci : nots) bytes += enc(ci);
+                for (uint32_t ci : cl.nots) bytes += enc(ci);
                 lp.postings += cost;
                 lp.algo_bytes += bytes;
                 // The lead is a block stream; every other term that has a score column is probed by one gather per
@@ -1372,12 +1421,12 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
                 if (range_lead) lp.clauses.push_back(range_clause(rreq[0].second, 0u));
                 for (size_t i = 0; i < req.size(); i++) put(req[i], i == 0 && !range_lead, 0u);
                 for (size_t i = range_lead ? 1 : 0; i < rreq.size(); i++) lp.clauses.push_back(range_clause(rreq[i].second, 0u));
-                for (uint32_t ci : nots) {
+                for (uint32_t ci : cl.nots) {
                     const int64_t col = col_of(columns, si, clauses[ci], k1bits);
                     if (col >= 0) lp.clauses.push_back(ItemClause{(uint32_t)col, 0.0f, clauses[ci].cache_id, kClauseNot | kClauseColumn});
                     else lp.clauses.push_back(ItemClause{clauses[ci].term_id, 0.0f, clauses[ci].cache_id, kClauseNot});
                 }
-                for (uint32_t ci : rnots) lp.clauses.push_back(range_clause(ci, kClauseNot));
+                for (uint32_t ci : cl.rnots) lp.clauses.push_back(range_clause(ci, kClauseNot));
                 for (const Req& r : opt) put(r, false, kClauseOpt);
                 const uint32_t n_item_terms = (uint32_t)(lp.clauses.size() - clause_begin);
                 if (n_item_terms > (uint32_t)kMaxTerms || (!range_lead && req[0].group && req[0].n > 8u))  // a leading group: one warp of k_eval_and_nested per member
@@ -1394,7 +1443,7 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
                 for (const Req& r : opt) grouped = grouped || r.group;
                 const bool ro = leaf_type == kTypeReqOpt;
                 const Route route = grouped                             ? (ro ? kRouteReqOptNested : kRouteAndNested)
-                                    : !rreq.empty() || !rnots.empty() ? (ro ? kRouteReqOptRanges : kRouteAndRanges)
+                                    : !rreq.empty() || !cl.rnots.empty() ? (ro ? kRouteReqOptRanges : kRouteAndRanges)
                                                                       : (ro ? kRouteReqOpt : kRouteAnd);
                 emit(route, leaf_type, n_item_terms, clause_begin, 0u, R, 1u, range_lead);
                 continue;
@@ -1606,50 +1655,92 @@ void plan_batch(rg_engine* e, const rg_query* queries, uint32_t n_queries, const
 }
 
 // The rescoring query's scorer per (query, leaf) for k_rescore (RescoreLeaf, engine.hpp), from the same shape
-// resolution as the first pass (classify + resolve_leaf).  Plans every query before anything is launched, so a
-// refused shape leaves the rows untouched.
+// classification and per-leaf resolution as the first pass (classify_batch, then ConjLeaf or resolve_leaf).  Plans
+// every query before anything is launched, so a refused shape leaves the rows untouched.
 struct RescorePlan {
     std::vector<RescoreLeaf> leaves;  // [n_queries][n_segs]
     std::vector<ItemClause> clauses;
+    std::vector<RangeRef> range_refs;  // per (leaf, range), when a query has ranges
+    bool nested = false;               // some clause is a group member or a range: k_rescore<true>
 };
 
 void plan_rescore(const rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
-                  uint32_t n_clauses, RescorePlan& rp) {
+                  uint32_t n_clauses, const rg_point_range* ranges, uint32_t n_ranges, const rg_query* groups,
+                  uint32_t n_groups, RescorePlan& rp) {
     const uint32_t n_caches = (uint32_t)(e->h_caches.size() / 256);
     const uint32_t n_segs = (uint32_t)e->segs.size();
+    std::vector<QShape> shapes;
+    std::vector<rg_clause> ext;
+    clauses = classify_batch(queries, n_queries, clauses, n_clauses, ranges, n_ranges, groups, n_groups, n_caches, true,
+                             ext, shapes);
     rp.leaves.assign((size_t)n_queries * n_segs, RescoreLeaf{0u, kRsNone, 0, 0, 0, 0.0f});
     rp.clauses.clear();
+    rp.range_refs.clear();
+    rp.nested = false;
+    if (has_ranges(shapes)) fill_range_refs(e, ranges, n_ranges, rp.range_refs);
     std::vector<uint32_t> present, nots, opts;
+    ConjLeaf cl;
     for (uint32_t qi = 0; qi < n_queries; qi++) {
-        QShape shape = classify(queries[qi], clauses, n_clauses, true);
-        // ReqNotScorer moves past an excluded hit with next(), and a SHOULD disjunction with min_should_match > 1
-        // then skips to the next doc that reaches min_should_match: whether a later hit matches depends on the walk
-        if (shape.msm > 1 && !shape.not_idx.empty())
-            throw Unsupported("rescoring with a min_should_match > 1 disjunction beside MUST_NOT clauses");
+        QShape& shape = shapes[qi];
         // advance() never counts clauses (disjunction_scorer.rs:350-364), and BooleanWeight::create_scorer builds the
         // DisjunctionSumScorer over whatever SHOULD clauses exist in the leaf, however few: min_should_match plays
         // no part in rescoring
         shape.msm = 0;
-        check_caches(shape, clauses, n_caches);
         // a bare TermQuery, or what BooleanQuery::build / DisjunctionMaxQuery::build collapse to one clause: the
         // TermScorer itself (a DisjunctionSumScorer would add it to 0.0f)
         const bool single = shape.type == kTypeOr && !shape.match_all && !shape.dismax && shape.clause_idx.size() == 1 &&
                             shape.not_idx.empty();
         for (uint32_t si = 0; si < n_segs; si++) {
-            if (!resolve_leaf(shape, e->segs[si], clauses, present, nots, opts)) continue;
+            const Segment& seg = e->segs[si];
             RescoreLeaf& L = rp.leaves[(size_t)qi * n_segs + si];
+            if (shape.type != kTypeOr) {
+                // a conjunction / ReqOptScorer, as the first pass resolves it: the required side in cost order (a
+                // range that leads first, the other required ranges after the terms and groups: each adds +0.0f), then
+                // the optional side in clause order, then the MUST_NOT terms and ranges
+                if (!cl.resolve(shape, seg, clauses, ranges)) continue;
+                L.clause_begin = (uint32_t)rp.clauses.size();
+                L.kind = kRsConj;
+                L.tie = shape.tie;
+                auto put = [&](const ConjLeaf::Req& r, uint32_t side) {
+                    for (uint32_t j = 0; j < r.n; j++) {
+                        const rg_clause& c = clauses[cl.members[r.begin + j]];
+                        if (r.group) {
+                            const uint32_t last = j + 1 == r.n ? kClauseGroupLast : 0u;
+                            rp.clauses.push_back(ItemClause{c.term_id, r.filter ? 0.0f : c.weight, c.cache_id,
+                                                            (side == kClauseOpt ? kClauseOptGroup : kClauseReqGroup) | last});
+                            rp.nested = true;
+                        } else {
+                            rp.clauses.push_back(ItemClause{c.term_id, clause_weight(c), c.cache_id, side});
+                        }
+                    }
+                };
+                auto range = [&](uint32_t ci, uint32_t not_flag) {
+                    rp.clauses.push_back(ItemClause{si * n_ranges + clauses[ci].term_id, 0.0f, 0u, kClauseRange | not_flag});
+                    rp.nested = true;
+                };
+                if (cl.range_lead) range(cl.rreq[0].second, 0u);
+                for (const ConjLeaf::Req& r : cl.req) put(r, 0u);
+                for (size_t i = cl.range_lead ? 1 : 0; i < cl.rreq.size(); i++) range(cl.rreq[i].second, 0u);
+                const size_t n_req = rp.clauses.size() - L.clause_begin;
+                for (const ConjLeaf::Req& r : cl.opt) put(r, kClauseOpt);
+                const size_t n_opt = rp.clauses.size() - L.clause_begin - n_req;
+                for (uint32_t ci : cl.nots) rp.clauses.push_back(ItemClause{clauses[ci].term_id, 0.0f, clauses[ci].cache_id, kClauseNot});
+                for (uint32_t ci : cl.rnots) range(ci, kClauseNot);
+                L.n_req = (uint8_t)n_req;
+                L.n_opt = (uint8_t)n_opt;
+                L.n_not = (uint8_t)(rp.clauses.size() - L.clause_begin - n_req - n_opt);
+                continue;
+            }
+            if (!resolve_leaf(shape, seg, clauses, present, nots, opts)) continue;
             L.clause_begin = (uint32_t)rp.clauses.size();
             if (shape.match_all) L.kind = kRsAll;
-            else if (shape.type != kTypeOr) L.kind = kRsConj;
             else if (shape.dismax) L.kind = present.size() > 1 ? kRsMax : kRsTerm;  // one scorer: that scorer (:135-155)
             else L.kind = single ? kRsTerm : kRsSum;
             L.tie = shape.tie;
             L.n_req = (uint8_t)present.size();
-            L.n_opt = (uint8_t)opts.size();
             L.n_not = (uint8_t)nots.size();
             for (uint32_t ci : present) rp.clauses.push_back(ItemClause{clauses[ci].term_id, clause_weight(clauses[ci]), clauses[ci].cache_id, 0u});
-            for (uint32_t ci : opts) rp.clauses.push_back(ItemClause{clauses[ci].term_id, clauses[ci].weight, clauses[ci].cache_id, 2u});
-            for (uint32_t ci : nots) rp.clauses.push_back(ItemClause{clauses[ci].term_id, 0.0f, clauses[ci].cache_id, 1u});
+            for (uint32_t ci : nots) rp.clauses.push_back(ItemClause{clauses[ci].term_id, 0.0f, clauses[ci].cache_id, kClauseNot});
         }
     }
 }
@@ -1668,7 +1759,8 @@ void queue_rescore(rg_engine* e, const RescorePlan& rp, DevBuf<uint8_t>& buf, co
                    const unsigned long long* d_totals) {
     cudaStream_t st = e->stream;
     const size_t leaves_b = (rp.leaves.size() * sizeof(RescoreLeaf) + 255) & ~(size_t)255;
-    const size_t total = leaves_b + std::max<size_t>(1, rp.clauses.size()) * sizeof(ItemClause);
+    const size_t clauses_b = (std::max<size_t>(1, rp.clauses.size()) * sizeof(ItemClause) + 255) & ~(size_t)255;
+    const size_t total = leaves_b + clauses_b + rp.range_refs.size() * sizeof(RangeRef);
     if (buf.n < total) buf.alloc(total);
     if (!rp.leaves.empty())
         RG_CUDA_CHECK(cudaMemcpyAsync(buf.p, rp.leaves.data(), rp.leaves.size() * sizeof(RescoreLeaf), cudaMemcpyHostToDevice,
@@ -1676,6 +1768,9 @@ void queue_rescore(rg_engine* e, const RescorePlan& rp, DevBuf<uint8_t>& buf, co
     if (!rp.clauses.empty())
         RG_CUDA_CHECK(cudaMemcpyAsync(buf.p + leaves_b, rp.clauses.data(), rp.clauses.size() * sizeof(ItemClause),
                                       cudaMemcpyHostToDevice, st));
+    if (!rp.range_refs.empty())
+        RG_CUDA_CHECK(cudaMemcpyAsync(buf.p + leaves_b + clauses_b, rp.range_refs.data(),
+                                      rp.range_refs.size() * sizeof(RangeRef), cudaMemcpyHostToDevice, st));
     RescoreParams rs{};
     rs.segs = e->d_segs.p;
     rs.n_segs = (uint32_t)e->segs.size();
@@ -1695,8 +1790,9 @@ void queue_rescore(rg_engine* e, const RescorePlan& rp, DevBuf<uint8_t>& buf, co
     uint32_t ncap = 32;
     while (ncap < std::min(k, p->window_size)) ncap <<= 1;
     rs.ncap = ncap;
+    rs.ranges = reinterpret_cast<const RangeRef*>(buf.p + leaves_b + clauses_b);
     RG_CUDA_CHECK(cudaEventRecord(e->rescore_ev[0], st));
-    launch_rescore(st, rs);
+    launch_rescore(st, rs, rp.nested);
     RG_CUDA_CHECK(cudaGetLastError());
     RG_CUDA_CHECK(cudaEventRecord(e->rescore_ev[1], st));
     e->rescore_timed = true;
@@ -2276,8 +2372,9 @@ int rg_merge_leaf_records(rg_engine* e, const void* dev_records_all, uint32_t n_
     RG_CATCH
 }
 
-int rg_batch_rescore(rg_engine* e, rg_batch* b, const rg_query* queries, uint32_t n_queries,
-                     const rg_clause* clauses, uint32_t n_clauses, const rg_rescore_params* p) {
+static int batch_rescore(rg_engine* e, rg_batch* b, const rg_query* queries, uint32_t n_queries,
+                         const rg_clause* clauses, uint32_t n_clauses, const rg_point_range* ranges, uint32_t n_ranges,
+                         const rg_query* groups, uint32_t n_groups, const rg_rescore_params* p) {
     RG_TRY
     if (!e || !b || !p || (n_queries && !queries) || (n_clauses && !clauses)) throw ArgError("null argument");
     check_rescore_params(p);
@@ -2288,7 +2385,7 @@ int rg_batch_rescore(rg_engine* e, rg_batch* b, const rg_query* queries, uint32_
     if (b->k > 1024) throw Unsupported("rows of more than 1024 hits are not accelerated");
     RG_CUDA_CHECK(cudaSetDevice(e->device));
     RescorePlan rp;
-    plan_rescore(e, queries, n_queries, clauses, n_clauses, rp);
+    plan_rescore(e, queries, n_queries, clauses, n_clauses, ranges, n_ranges, groups, n_groups, rp);
     queue_rescore(e, rp, b->rescore_plan, p, n_queries, b->k, b->out_hits.p, b->out_counts.p, b->out_total.p);
     RG_CUDA_CHECK(cudaEventRecord(b->done, e->stream));  // rg_batch_fetch waits for the rescored rows
     b->synced = false;
@@ -2296,9 +2393,10 @@ int rg_batch_rescore(rg_engine* e, rg_batch* b, const rg_query* queries, uint32_
     RG_CATCH
 }
 
-int rg_rescore_hits(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
-                    uint32_t n_clauses, const rg_rescore_params* p, uint32_t k, rg_hit* hits,
-                    const uint32_t* counts, const uint64_t* total_hits) {
+static int rescore_hits(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                        uint32_t n_clauses, const rg_point_range* ranges, uint32_t n_ranges, const rg_query* groups,
+                        uint32_t n_groups, const rg_rescore_params* p, uint32_t k, rg_hit* hits, const uint32_t* counts,
+                        const uint64_t* total_hits) {
     RG_TRY
     if (!e || !p || (n_queries && (!queries || !hits || !counts || !total_hits)) || (n_clauses && !clauses))
         throw ArgError("null argument");
@@ -2318,7 +2416,7 @@ int rg_rescore_hits(rg_engine* e, const rg_query* queries, uint32_t n_queries, c
     RG_CUDA_CHECK(cudaSetDevice(e->device));
     e->sync_tables();
     RescorePlan rp;
-    plan_rescore(e, queries, n_queries, clauses, n_clauses, rp);
+    plan_rescore(e, queries, n_queries, clauses, n_clauses, ranges, n_ranges, groups, n_groups, rp);
     if (n_queries == 0) return RG_OK;
     const size_t hits_b = ((size_t)n_queries * k * sizeof(rg_hit) + 255) & ~(size_t)255;
     const size_t counts_b = ((size_t)n_queries * 4 + 255) & ~(size_t)255;
@@ -2336,6 +2434,34 @@ int rg_rescore_hits(rg_engine* e, const rg_query* queries, uint32_t n_queries, c
     RG_CUDA_CHECK(cudaStreamSynchronize(st));
     return RG_OK;
     RG_CATCH
+}
+
+int rg_batch_rescore(rg_engine* e, rg_batch* b, const rg_query* queries, uint32_t n_queries,
+                     const rg_clause* clauses, uint32_t n_clauses, const rg_rescore_params* p) {
+    return batch_rescore(e, b, queries, n_queries, clauses, n_clauses, nullptr, 0, nullptr, 0, p);
+}
+
+int rg_batch_rescore_nested(rg_engine* e, rg_batch* b, const rg_query* queries, uint32_t n_queries,
+                            const rg_clause* clauses, uint32_t n_clauses, const rg_point_range* ranges,
+                            uint32_t n_ranges, const rg_query* groups, uint32_t n_groups, const rg_rescore_params* p) {
+    if (!readable(ranges, n_ranges) || !readable(groups, n_groups)) return null_argument(nullptr);
+    return batch_rescore(e, b, queries, n_queries, clauses, n_clauses, ranges, n_ranges, groups, n_groups, p);
+}
+
+int rg_rescore_hits(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                    uint32_t n_clauses, const rg_rescore_params* p, uint32_t k, rg_hit* hits,
+                    const uint32_t* counts, const uint64_t* total_hits) {
+    return rescore_hits(e, queries, n_queries, clauses, n_clauses, nullptr, 0, nullptr, 0, p, k, hits, counts,
+                        total_hits);
+}
+
+int rg_rescore_hits_nested(rg_engine* e, const rg_query* queries, uint32_t n_queries, const rg_clause* clauses,
+                           uint32_t n_clauses, const rg_point_range* ranges, uint32_t n_ranges, const rg_query* groups,
+                           uint32_t n_groups, const rg_rescore_params* p, uint32_t k, rg_hit* hits,
+                           const uint32_t* counts, const uint64_t* total_hits) {
+    if (!readable(ranges, n_ranges) || !readable(groups, n_groups)) return null_argument(nullptr);
+    return rescore_hits(e, queries, n_queries, clauses, n_clauses, ranges, n_ranges, groups, n_groups, p, k, hits,
+                        counts, total_hits);
 }
 
 // ncclAllGather, resolved at run time so that librucene_gpu.so carries no link-time NCCL dependency (a PyTorch

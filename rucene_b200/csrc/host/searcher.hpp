@@ -270,14 +270,21 @@ public:
         std::vector<ScoreDoc>& docs = top_docs.score_docs_mut();
         if (top_docs.total_hits() == 0 || docs.empty()) return;  // rescorer.rs:548-550
         std::vector<rg_clause> clauses;
-        rg_query q = compile(query, clauses);
+        std::vector<rg_point_range> ranges;
+        std::vector<rg_query> groups;
+        rg_query q = compile(query, clauses, &ranges, &groups);
         std::vector<rg_hit> hits(docs.size());
         for (size_t i = 0; i < docs.size(); i++) hits[i] = rg_hit{docs[i].doc, docs[i].score};
         const uint32_t count = (uint32_t)docs.size();
         const uint64_t total = top_docs.total_hits();
         rg_rescore_params p{window_size, query_weight, rescore_weight, mode, sim_.k1, 0};
-        check(rg_rescore_hits(engine_, &q, 1, clauses.data(), (uint32_t)clauses.size(), &p, count, hits.data(), &count,
-                              &total));
+        if (groups.empty() && ranges.empty())
+            check(rg_rescore_hits(engine_, &q, 1, clauses.data(), (uint32_t)clauses.size(), &p, count, hits.data(),
+                                  &count, &total));
+        else
+            check(rg_rescore_hits_nested(engine_, &q, 1, clauses.data(), (uint32_t)clauses.size(), ranges.data(),
+                                         (uint32_t)ranges.size(), groups.data(), (uint32_t)groups.size(), &p, count,
+                                         hits.data(), &count, &total));
         for (size_t i = 0; i < docs.size(); i++) docs[i] = ScoreDoc{hits[i].doc, hits[i].score};
     }
 
@@ -328,7 +335,7 @@ private:
         }
         auto pq = dynamic_cast<const PointRangeQuery*>(&leaf);
         if (!pq) throw UnsupportedQuery("only TermQuery and PointRangeQuery leaves are accelerated");
-        if (!ranges) throw UnsupportedQuery("PointRangeQuery is not accelerated here (rescoring)");
+        if (!ranges) throw UnsupportedQuery("PointRangeQuery is not accelerated here");
         rg_point_range r{};
         auto it = point_fields_.find(pq->field);
         r.field = it == point_fields_.end() ? 0xffffffffu : it->second;  // no leaf has points of it: no scorer anywhere

@@ -118,6 +118,10 @@ def lib():
     L.rg_batch_rescore.argtypes = [vp, vp, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(RescoreParams)]
     L.rg_rescore_hits.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, C.POINTER(RescoreParams), C.c_uint32, vp, vp,
                                   vp]
+    L.rg_batch_rescore_nested.argtypes = [vp, vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32,
+                                          C.POINTER(RescoreParams)]
+    L.rg_rescore_hits_nested.argtypes = [vp, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32, vp, C.c_uint32,
+                                         C.POINTER(RescoreParams), C.c_uint32, vp, vp, vp]
     L.rg_segment_decode.argtypes = [vp, C.c_uint32, C.c_uint64, C.c_uint64, vp, vp]
     L.rg_forutil_decode.argtypes = [vp, vp, C.c_size_t, vp, C.c_uint32, C.c_int, vp, vp]
     L.rg_blockset_stage.argtypes = [vp, vp, C.c_size_t, vp, C.c_uint32, C.c_int, vp, C.POINTER(vp)]
@@ -420,25 +424,43 @@ class Engine:
     def _rescore_params(window_size, query_weight, rescore_weight, mode, k1):
         return RescoreParams(min(int(window_size), 0xFFFFFFFF), query_weight, rescore_weight, mode, k1, 0)
 
+    @staticmethod
+    def _nested_arrays(groups, ranges):
+        g = None if groups is None else np.ascontiguousarray(groups, dtype=QUERY_DTYPE)
+        r = None if ranges is None else np.ascontiguousarray(ranges, dtype=RANGE_DTYPE)
+        return g, r, 0 if g is None else len(g), 0 if r is None else len(r)
+
     def rescore_batch(self, batch, queries, clauses, window_size, query_weight=1.0, rescore_weight=1.0,
-                      mode=RESCORE_TOTAL, k1=1.2):
-        """rg_batch_rescore: after batch.run(), before batch.fetch(); rescores the batch's rows on the device."""
+                      mode=RESCORE_TOTAL, k1=1.2, groups=None, ranges=None):
+        """rg_batch_rescore: after batch.run(), before batch.fetch(); rescores the batch's rows on the device.
+        groups / ranges (the rescoring queries' own arrays, either may be None): rg_batch_rescore_nested."""
         q = np.ascontiguousarray(queries, dtype=QUERY_DTYPE)
         c = np.ascontiguousarray(clauses, dtype=CLAUSE_DTYPE)
         p = self._rescore_params(window_size, query_weight, rescore_weight, mode, k1)
-        _check(lib().rg_batch_rescore(self.h, batch.h, _p(q), len(q), _p(c), len(c), C.byref(p)), self.h)
+        if groups is None and ranges is None:
+            _check(lib().rg_batch_rescore(self.h, batch.h, _p(q), len(q), _p(c), len(c), C.byref(p)), self.h)
+            return
+        g, r, ng, nr = self._nested_arrays(groups, ranges)
+        _check(lib().rg_batch_rescore_nested(self.h, batch.h, _p(q), len(q), _p(c), len(c), _p(r), nr, _p(g), ng,
+                                             C.byref(p)), self.h)
 
     def rescore_hits(self, queries, clauses, hits, counts, total, window_size, query_weight=1.0, rescore_weight=1.0,
-                     mode=RESCORE_TOTAL, k1=1.2):
-        """rg_rescore_hits over host rows (hits [n, k] of HIT_DTYPE); returns the rescored copy of hits."""
+                     mode=RESCORE_TOTAL, k1=1.2, groups=None, ranges=None):
+        """rg_rescore_hits over host rows (hits [n, k] of HIT_DTYPE); returns the rescored copy of hits.
+        groups / ranges (either may be None): rg_rescore_hits_nested."""
         q = np.ascontiguousarray(queries, dtype=QUERY_DTYPE)
         c = np.ascontiguousarray(clauses, dtype=CLAUSE_DTYPE)
         h = np.array(hits, dtype=HIT_DTYPE, copy=True, order="C").reshape(len(q), -1)
         n = np.ascontiguousarray(counts, dtype=np.uint32)
         t = np.ascontiguousarray(total, dtype=np.uint64)
         p = self._rescore_params(window_size, query_weight, rescore_weight, mode, k1)
-        _check(lib().rg_rescore_hits(self.h, _p(q), len(q), _p(c), len(c), C.byref(p), h.shape[1], _p(h), _p(n),
-                                     _p(t)), self.h)
+        if groups is None and ranges is None:
+            _check(lib().rg_rescore_hits(self.h, _p(q), len(q), _p(c), len(c), C.byref(p), h.shape[1], _p(h), _p(n),
+                                         _p(t)), self.h)
+            return h
+        g, r, ng, nr = self._nested_arrays(groups, ranges)
+        _check(lib().rg_rescore_hits_nested(self.h, _p(q), len(q), _p(c), len(c), _p(r), nr, _p(g), ng, C.byref(p),
+                                            h.shape[1], _p(h), _p(n), _p(t)), self.h)
         return h
 
     def merge_leaf_records(self, dev_ptr, n_leaves, n_queries, k):

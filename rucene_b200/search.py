@@ -253,13 +253,13 @@ class QueryRescorer:
         docs = top_docs.score_docs()
         if top_docs.total_hits() == 0 or not docs:
             return
-        q, c = searcher.compile_batch([request.query])
+        q, c, ranges, groups = searcher._compile_any([request.query])
         hits = np.zeros((1, len(docs)), engine.HIT_DTYPE)
         hits[0]["doc"] = [d.doc for d in docs]
         hits[0]["score"] = np.array([d.score for d in docs], np.float32)
         out = searcher.engine.rescore_hits(q, c, hits, [len(docs)], [top_docs.total_hits()], request.window_size,
                                            request.query_weight, request.rescore_weight, int(request.mode),
-                                           k1=searcher.similarity.k1)
+                                           k1=searcher.similarity.k1, groups=groups, ranges=ranges)
         for i, h in enumerate(out[0]):
             docs[i].doc = int(h["doc"])
             docs[i].score = float(h["score"])
@@ -531,16 +531,19 @@ class GpuIndexSearcher:
             return False
         return any(walk(q) for q in queries)
 
+    def _compile_any(self, queries):
+        """(queries, clauses, ranges, groups) through the compile call the batch needs; ranges / groups None when
+        the plain or the *_ranges calls take it"""
+        if self._has_groups(queries):
+            return self.compile_batch_nested(queries)
+        if self._has_ranges(queries):
+            return self.compile_batch_ranges(queries) + (None,)
+        return self.compile_batch(queries) + (None, None)
+
     def search_batch(self, queries, k, mode=engine.MODE_SEARCH, rescore=None):
         """rescore: (rescoring queries, RescoreRequest) — one rescoring query per query, the request's weights,
         mode and window for all: QueryRescorer::rescore on every row on the device before the rows are fetched."""
-        ranges = groups = None
-        if self._has_groups(queries):
-            q, c, ranges, groups = self.compile_batch_nested(queries)
-        elif self._has_ranges(queries):
-            q, c, ranges = self.compile_batch_ranges(queries)
-        else:
-            q, c = self.compile_batch(queries)
+        q, c, ranges, groups = self._compile_any(queries)
         if rescore is None:
             if groups is not None:
                 return self.engine.search_batch_nested(q, c, groups, k, k1=self.similarity.k1, mode=mode,
@@ -549,12 +552,12 @@ class GpuIndexSearcher:
                 return self.engine.search_batch_ranges(q, c, ranges, k, k1=self.similarity.k1, mode=mode)
             return self.engine.search_batch(q, c, k, k1=self.similarity.k1, mode=mode)
         rescore_queries, req = rescore
-        rq, rc = self.compile_batch(rescore_queries)   # rescoring takes no ranges: a PointRangeQuery is refused
+        rq, rc, rranges, rgroups = self._compile_any(rescore_queries)   # their own range / group arrays
         batch = self.engine.prepare(q, c, k, k1=self.similarity.k1, mode=mode, ranges=ranges, groups=groups)
         try:
             batch.run()
             self.engine.rescore_batch(batch, rq, rc, req.window_size, req.query_weight, req.rescore_weight,
-                                      int(req.mode), k1=self.similarity.k1)
+                                      int(req.mode), k1=self.similarity.k1, groups=rgroups, ranges=rranges)
             return batch.fetch()
         finally:
             batch.close()
